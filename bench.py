@@ -39,6 +39,8 @@ def parse():
     ap.add_argument("--no-literal", action="store_true", help="skip the extra measurement with dead-frame elimination off")
     ap.add_argument("--cpu-frames", type=int, default=4, help="frames in the bounded CPU sample")
     ap.add_argument("--no-extra", action="store_true", help="skip the secondary configs (100-step inference, N_res=1024)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -134,11 +136,10 @@ def pick_host_threads():
 
 
 def _reference_root():
-    """Where an unmodified reference checkout is importable from (never on the GPU box unless the driver installed
-    one under baseline/_ref)."""
-    for cand in (os.environ.get("DFOLD_REFERENCE_ROOT"), os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
-        if cand and os.path.isdir(os.path.join(cand, "src", "model")):
-            return cand
+    """Where an unmodified reference checkout is importable from: $DFOLD_REFERENCE_ROOT, if set."""
+    cand = os.environ.get("DFOLD_REFERENCE_ROOT")
+    if cand and os.path.isdir(os.path.join(cand, "src", "model")):
+        return cand
     return None
 
 
@@ -250,7 +251,7 @@ def _log(msg):
 
 def time_ipa_core(dev, nf, N, iters=20):
     """Fused IPA forward core alone at the benchmark shape (preset A), CUDA events on the launching stream around `iters`
-    back-to-back calls after 3 warm-up calls.  Inputs (q/k/v, points, pair, bias: 659 MB at nf=64) exceed the 126 MB L2."""
+    back-to-back calls after 3 warm-up calls.  Inputs (q/k/v, points, pair, bias: 659 MB at nf=64) exceed the 50 MB L2."""
     from dynamicpdb_b200 import kernels as K
     H, C, Pq, Pv, Cp = 8, 256, 8, 12, 32
     g = torch.Generator(device=dev).manual_seed(0)
@@ -474,6 +475,8 @@ def run_ours(args):
         sampler.start()
     ms = timed(args.steps, e2e=False)
     _log(f"timed region done: {ms:.1f} ms/step")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ts)
     ms_e2e = timed(args.steps, e2e=True)
     _log("e2e region done")
     clocks = sampler.stop() if sampler else None
@@ -515,13 +518,8 @@ def run_ours(args):
     except Exception:
         pass
     tf_peak, tf_src = (peaks.get("bf16_tflops_sustained"), "measured (sustained)") if peaks.get("bf16_tflops_sustained") \
-        else (1400.0, "fallback")
-    hbm_peak, hbm_src = (peaks.get("hbm_gbs"), "measured") if peaks.get("hbm_gbs") else (6650.0, "fallback")
-    traffic = {}
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    except Exception:
-        pass
+        else (989.0, "H100 SXM data sheet, dense BF16 at 700 W")
+    hbm_peak, hbm_src = (peaks.get("hbm_gbs"), "measured") if peaks.get("hbm_gbs") else (3350.0, "H100 SXM data sheet")
     agg = {}
     for name, work, a, b, _tag in prof:
         t = a.elapsed_time(b) * 1e-3
@@ -535,8 +533,7 @@ def run_ours(args):
         ach = w / t / 1e12
         roof = {"kernel": "gemm_bf16x3_kernel (implicit 5x5 conv / linear, 3 bf16 MMAs per fp32 product)",
                 "bound": "tensor", "achieved": ach, "peak": tf_peak, "unit": "TFLOP/s", "frac": ach / tf_peak,
-                "peak_source": tf_src, "traffic": traffic.get("gemm_dram_bytes_per_launch"),
-                "traffic_note": traffic.get("gemm_note"), "launches_timed": n, "avg_launch_ms": 1e3 * t / n,
+                "peak_source": tf_src, "launches_timed": n, "avg_launch_ms": 1e3 * t / n,
                 "share_of_step": (t / prof_steps) / (ms * 1e-3), "tensor_pipe_frac": 3 * ach / tf_peak,
                 "timed_in": "eager instrumented steps right after the timed (graph-replayed) region",
                 "note": "achieved counts fp32-equivalent FLOPs; the split issues 3 bf16 MMAs per product, so frac <= 1/3"}
@@ -549,9 +546,9 @@ def run_ours(args):
             w, t, n = agg["ipa_fwd"]
             in_step = {"launches_timed": n, "avg_ms_eager_events": 1e3 * t / n,
                        "note": "event pairs around the op inside the eager instrumented steps; includes host launch gaps"}
-        roof_ipa = {"kernel": "ipa_fused_fwd_kernel + tcgen05 P.V (fused IPA forward core, SURVEY.md 8d)", "bound": "hbm",
+        roof_ipa = {"kernel": "ipa_fused_fwd_kernel + P.V GEMM (fused IPA forward core, SURVEY.md 8d)", "bound": "hbm",
                     "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "peak_source": hbm_src,
-                    "traffic": traffic.get("ipa_fwd_dram_bytes_per_launch"), "algorithmic_bytes": ipa_alg,
+                    "algorithmic_bytes": ipa_alg,
                     "avg_launch_ms": ipa_ms, "inference_ms": ipa_infer_ms, "kernels_per_call": ipa_launches, "calls_per_step": 4,
                     "share_of_step": 4 * ipa_ms / ms, "in_step": in_step,
                     "timed_in": "20 back-to-back calls of the op at the benchmark shape, CUDA events on the launching stream, "
@@ -578,10 +575,11 @@ def run_ours(args):
     line = {
         "metric": METRIC, "value": world * nf / (ms * 1e-3), "unit": "frames/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": "f32 (bf16x3 split on tcgen05, fp32 accumulate)", "data": "synthetic",
+        "dtype": "f32 (bf16x3 split on wgmma, fp32 accumulate)", "data": "synthetic",
         "config": {"workload": f"DFOLDv2 training step fwd+bwd+Adam, N_res={N}, batch={nf} frames per rank (configs[2])",
                    "frames_per_rank": nf, "n_res": N, "preset": "train_DFOLDv2.yaml (c_s 256, c_z 128, C 256, H 8, Pq 8, Pv 12, 4 blocks)",
-                   "parallelism": f"dp{world}", "l2": "working set (weights 738 MB + activations) exceeds the 126 MB L2",
+                   "parallelism": f"dp{world}", "l2": "working set (weights 738 MB + activations) exceeds the 50 MB L2",
+                   "gpu": torch.cuda.get_device_name(dev),
                    "cuda_graph": graph_on, "cuda_graph_error": graph_err,
                    "dead_frame_elimination": os.environ.get("DFOLD_NO_DEAD_FRAME_SKIP", "0") != "1"},
         "e2e": {"value": world * nf / (ms_e2e * 1e-3), "unit": "frames/s", "ms_per_step": ms_e2e,
@@ -591,6 +589,29 @@ def run_ours(args):
     }
     print(json.dumps(line), file=_REAL_STDOUT, flush=True)
     _finish(world, dist)
+
+
+DUMP_SAMPLE = 1 << 21      # elements kept of each flat parameter-sized array
+
+
+def dump_outputs(out_dir, ts):
+    """What the last timed step handed back, as float32 / float64 .npy files: the loss it returns, and the updated
+    parameters and gradients it leaves in place, as a fixed seeded sample of 2^21 positions of the flat arrays (their
+    indices in `flat_index.npy`) -- 32 MB in all.  The inputs are seeded, so two builds run with the same arguments can
+    be compared array for array."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    params = torch.cat([p.detach().reshape(-1) for p in ts.params])
+    grads = torch.cat([(p.grad if p.grad is not None else torch.zeros_like(p)).detach().reshape(-1) for p in ts.params])
+    n = params.numel()
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randint(0, n, (min(n, DUMP_SAMPLE),), generator=g).sort().values
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(ts.loss)], dtype=np.float64))
+    np.save(os.path.join(out_dir, "flat_index.npy"), idx.double().numpy())
+    np.save(os.path.join(out_dir, "params_sample.npy"), params[idx.to(params.device)].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "grads_sample.npy"), grads[idx.to(grads.device)].float().cpu().numpy())
+    del params, grads
 
 
 def _finish(world, dist):

@@ -1,2 +1,2 @@
-"""dynamicpdb_b200: B200-native DFOLDv2 score-network hot path (see DESIGN.md)."""
+"""dynamicpdb_b200: H100-native (sm_90a) DFOLDv2 score-network hot path (see DESIGN.md)."""
 __version__ = "0.1.0"

@@ -1,4 +1,4 @@
-"""Build libdfold_b200.so (sm_100a) in-tree with nvcc.  Used by __graft_entry__.build() and `python -m dynamicpdb_b200.build`."""
+"""Build libdfold_b200.so (sm_90a) in-tree with nvcc.  Used by __graft_entry__.build() and `python -m dynamicpdb_b200.build`."""
 import os
 import subprocess
 import sys
@@ -6,9 +6,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdfold_b200.so")
-SOURCES = ["simt.cu", "rigid.cu", "epilogue.cu", "loss.cu", "featurize.cu", "ipa_attn.cu", "ipa_v2.cu", "ipa_fused.cu", "gemm_sm100.cu"]
+SOURCES = ["simt.cu", "rigid.cu", "epilogue.cu", "loss.cu", "featurize.cu", "ipa_attn.cu", "ipa_v2.cu", "ipa_fused.cu", "gemm_sm90.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -40,7 +40,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(f"[dfold build] {s}:\n{out}\n")
     if not ok:
         raise RuntimeError("nvcc failed")
-    subprocess.check_call([NVCC, "-shared", "-o", LIB, *objs, "-cudart", "static"])
+    subprocess.check_call([NVCC, *FLAGS[:2], "-shared", "-o", LIB, *objs, "-cudart", "static"])
     return LIB
 
 

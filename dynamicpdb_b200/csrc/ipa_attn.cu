@@ -1,4 +1,4 @@
-// Fused invariant-point-attention core for sm_100a.
+// Fused invariant-point-attention core for sm_90a.
 //
 // One kernel does: scalar logits (+pair bias, precomputed by the tensor-core GEMM) + point-distance term on
 // coordinate DIFFERENCES + mask + online softmax + value / value-point / pair aggregation + local-frame
@@ -411,7 +411,7 @@ __global__ void __launch_bounds__(256) ipa_bwd_row_kernel(const IpaParams p, con
     if (tid == 0) {
         float t = 0.f;
         for (int w = 0; w < 8; ++w) t += s_red[w];
-        atomicAdd(dgamma + h, t);
+        dgamma[(long)h * p.F * p.N + (long)blockIdx.z * gridDim.x + blockIdx.x] = t;   // per-CTA partial (no atomics)
     }
 }
 

@@ -1,23 +1,19 @@
-// Fused invariant-point-attention forward core for the frame-shared (DFOLDv2) case, sm_100a.
+// Fused invariant-point-attention forward core for the frame-shared (DFOLDv2) case, sm_90a.
 //
-// One CTA = (32 query residues, one trajectory frame, all 8 heads), 16 compute warps (+ 1 control warp in the
-// tensor-core variant).  Per CTA, over key tiles of 32 residues:
+// One CTA = (32 query residues, one trajectory frame, all 8 heads), 16 warps.  Per CTA, over key tiles of 32 residues:
 //   pass 1   exact softmax statistics (row max m, row sum l) of
 //                s[h,i,j] = logit0[h,i,j] - gamma_h/2 * sum_p |q_p(i) - k_p(j)|^2 + inf * (mask_i mask_j - 1)
-//            with the coordinate differences in exact fp32 (packed FADD2 / FFMA2): key points arrive by TMA (double-buffered
-//            tiles), each lane keeps one key in registers, the query points are broadcast from shared memory, (m, l) are
-//            kept online per lane and combined by warp shuffles at the end -- no whole-row shared memory, no cap on N;
-//   pass 2   per key tile: (A) p = exp(s - m) / l, written once to shared memory (fp32, all heads), to the bf16
-//            hi/lo planes P[F,H,N,ldp] that the backward GEMMs read, and (tensor-core variant) to a 128B-swizzled
-//            bf16 hi/lo operand tile; (B1) pair aggregation o_pair[i,h,:] += p[h,i,j] z[i,j,:] with lanes across the
+//            with the coordinate differences in exact fp32: key points arrive by TMA (double-buffered tiles), each lane
+//            keeps one key in registers, the query points are broadcast from shared memory, (m, l) are kept online per
+//            lane and combined by warp shuffles at the end -- no whole-row shared memory, no cap on N;
+//   pass 2   per key tile: (A) p = exp(s - m) / l, written once to shared memory (fp32, all heads) and to the bf16
+//            hi/lo planes P[F,H,N,ldp]; (B1) pair aggregation o_pair[i,h,:] += p[h,i,j] z[i,j,:] with lanes across the
 //            pair channels, z read once from L2 for all 8 heads; (B2) value-point aggregation
 //            o_pt[h,i,:] += p[h,i,j] v_pts[j,h,:] with the tile's value points landing as one TMA box;
-//   P V      tensor-core variant: the control warp streams V^T tiles (MN-major, straight from the [N, H*2C] bf16 planes
-//            of kv) through a TMA / mbarrier ring and issues tcgen05.mma  O^T[c, i] += V^T[c, j] P^T[j, i]  (M = 128 c,
-//            N = 32 rows, hi*hi + hi*lo + lo*hi) into 16 TMEM accumulators (8 heads x 2 halves of C = 256) = all 512
-//            columns; P never leaves the SM on its way to P V.  Without V planes the scalar values are left to
-//            dfold_gemm_bf16x3_batched over the probability planes.
-//   epilogue local-frame transform R_i^T (o_pt - t_i), norms, reference concat layout, coalesced stores; TMEM -> o columns.
+//   epilogue local-frame transform R_i^T (o_pt - t_i), norms, reference concat layout, coalesced stores.
+// The scalar values O = P V are left to dfold_gemm_bf16x3_batched over the probability planes: one CTA's accumulator
+// (8 heads x 256 channels x 32 rows in fp32 = 256 KB) fits neither the register file next to the 16 warps' state nor
+// shared memory on sm_90.
 //
 // Reference: src/model/ipa_pytorch_dynamic.py:402-504 (logits :402-447, softmax :448, aggregations :455-504).
 #include <cuda.h>
@@ -35,7 +31,6 @@ constexpr int FTJ = 32;      // keys per tile
 constexpr int FPQ = 8;       // query / key points
 constexpr int FPV = 12;      // value points
 constexpr int FCP = 32;      // pair channels (c_z / 4)
-constexpr int FC = 256;      // scalar value channels per head (tensor-core variant)
 constexpr int PQ3 = FPQ * 3; // 24
 constexpr int PV3 = FPV * 3; // 36
 constexpr int FW = PQ3 + PV3;
@@ -57,23 +52,29 @@ struct FusedParams {
     int F, N, C, dfold;
     float inf, eps;
     long long* stats;                      // development aid (dfold_debug_ipa_stats): 16 x int64 cycle counters per CTA
-    int skip;                              // development knob (DFOLD_IPA_DEBUG_SKIP): bit 0 pass 1, 1 distances, 2 B1, 3 B2, 4 MMA
+    int skip;                              // development knob (DFOLD_IPA_DEBUG_SKIP): bit 0 pass 1, 1 distances, 2 B1, 3 B2
 };
 
 __device__ __forceinline__ u64 pack2(float a, float b) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
 __device__ __forceinline__ void unpack2(u64 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ u64 sub2(u64 a, u64 b) { u64 r; asm("sub.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) { u64 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
+// coordinate pairs held as 64-bit words; sm_90 has no packed FP32 arithmetic, so each pair op is two scalar rn ops
+__device__ __forceinline__ u64 sub2(u64 a, u64 b) {
+    float a0, a1, b0, b1;
+    unpack2(a, a0, a1); unpack2(b, b0, b1);
+    return pack2(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
+}
+__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
+    float a0, a1, b0, b1, c0, c1;
+    unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
+    return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
+}
 __device__ __forceinline__ float ex2f(float x) { float r; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
-__device__ __forceinline__ void comp_sync() { asm volatile("bar.sync 1, 512;" ::: "memory"); }   // the 16 compute warps
+__device__ __forceinline__ void comp_sync() { asm volatile("bar.sync 1, 512;" ::: "memory"); }   // the 16 warps
 
-// ---- tcgen05 / TMA / mbarrier wrappers (same forms as csrc/gemm_sm100.cu) ----
+// ---- TMA / mbarrier wrappers (same forms as csrc/gemm_sm90.cu) ----
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -94,54 +95,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
         "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
         ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(bar) : "memory");
 }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// K-major, 128B-swizzled operand tile (rows of 128 B, 8-row groups 1024 B apart)
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-// MN-major, 128B-swizzled operand tile stored [k][mn]: 64 mn elements (128 B) per k row, 8 k rows per 1024 B atom (SBO),
-// the next 64-wide mn atom `lbo` bytes further (32 k rows x 128 B here)
-__device__ __forceinline__ uint64_t make_sw128_mn_desc(uint32_t smem_addr, uint32_t lbo) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)(lbo >> 4) << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
 // squared distance summed over the 8 point pairs: q (shared memory, broadcast) against the lane's key in registers
 __device__ __forceinline__ float dist2(const ulonglong2* __restrict__ q2, const u64 (&k)[12]) {
     ulonglong2 qq[6];
@@ -190,136 +143,34 @@ constexpr int SST = 772;                       // staging row stride (floats): 1
 constexpr int kStage = FTI * SST;              // epilogue staging of the point features
 constexpr int kSK = FTJ * FH * PQ3;             // key points of a tile [h][j][24] (8 TMA boxes): pass 1, in the s_v / s_p space
 constexpr int kWork = kSQ + kSV + kSP;
-constexpr int kPB = 65536;                     // tensor-core variant: bf16 P tiles  [h][hi|lo][32 rows][128 B]   (bytes)
-constexpr int kRingStage = 16384;              //   one V^T stage: [hi|lo][2 mn atoms][32 k rows][128 B]           (bytes)
-constexpr int kRingStages = 4;
-constexpr int kRing = kRingStages * kRingStage;
+// [max(work, stage) | row | stat | barriers]: the epilogue stages in the work space
+constexpr int kWorkFloats = kWork > kStage + FH * FTI * PV3 ? kWork : kStage + FH * FTI * PV3;
+constexpr int kFusedBytes = 4 * (kWorkFloats + kSRow + kSStat) + 64 + 1024;      // + barriers + alignment slack
 
-template <bool TC> struct FCfg {
-    static constexpr int kThreads = TC ? NCOMP + 32 : NCOMP;
-    // TC: [pb | ring | work | row | stat | barriers], the epilogue stages in pb/ring;  else: [max(work, stage) | row | stat]
-    static constexpr int kFloatBase = TC ? (kPB + kRing) : 0;                                   // bytes
-    static constexpr int kWorkFloats = TC ? kWork : (kWork > kStage + FH * FTI * PV3 ? kWork : kStage + FH * FTI * PV3);
-    static constexpr int kBytes = kFloatBase + 4 * (kWorkFloats + kSRow + kSStat) + 192 + 1024;     // + barriers + alignment slack
-};
-
-template <bool TC>
-__global__ void __launch_bounds__(FCfg<TC>::kThreads, 1)
-ipa_fused_fwd_kernel(const FusedParams p, const __grid_constant__ CUtensorMap map_v_hi, const __grid_constant__ CUtensorMap map_v_lo,
-                     const __grid_constant__ CUtensorMap map_pts, const __grid_constant__ CUtensorMap map_kpt) {
-    using Cfg = FCfg<TC>;
+__global__ void __launch_bounds__(NCOMP, 1)
+ipa_fused_fwd_kernel(const FusedParams p, const __grid_constant__ CUtensorMap map_pts, const __grid_constant__ CUtensorMap map_kpt) {
     extern __shared__ __align__(16) unsigned char sm_raw[];
     unsigned char* sm_base = sm_raw;
-    sm_base = sm_raw + ((1024u - (smem_u32(sm_raw) & 1023u)) & 1023u);      // TMA / UMMA tiles want 128 B / 1024 B alignment
-    float* smf = reinterpret_cast<float*>(sm_base + Cfg::kFloatBase);
+    sm_base = sm_raw + ((1024u - (smem_u32(sm_raw) & 1023u)) & 1023u);      // TMA boxes want 128 B alignment
+    float* smf = reinterpret_cast<float*>(sm_base);
     float* s_q = smf;
     float* s_v = s_q + kSQ;
     float* s_p = s_v + kSV;
-    float* s_row = smf + Cfg::kWorkFloats;
+    float* s_row = smf + kWorkFloats;
     float* s_stat = s_row + kSRow;
-    float* stage = TC ? reinterpret_cast<float*>(sm_base) : smf;
-    const uint32_t pb_u32 = smem_u32(sm_base);
-    const uint32_t ring_u32 = pb_u32 + kPB;
+    float* stage = smf;
     const uint32_t bar_u32 = smem_u32(s_stat + kSStat);
-    // barriers (TC): full[4], empty[4], p_ready[2], p_free[2], acc_done, then the TMEM pointer word
-    auto full_bar = [&](int s) { return bar_u32 + 8u * s; };
-    auto empty_bar = [&](int s) { return bar_u32 + 8u * (kRingStages + s); };
-    auto pready_bar = [&](int b) { return bar_u32 + 8u * (2 * kRingStages + b); };
-    auto pfree_bar = [&](int b) { return bar_u32 + 8u * (2 * kRingStages + 2 + b); };
-    const uint32_t accdone_bar = bar_u32 + 8u * (2 * kRingStages + 4);
-    const uint32_t tmem_slot = bar_u32 + 8u * (2 * kRingStages + 5);
-    const uint32_t vfull_bar = bar_u32 + 8u * (2 * kRingStages + 6);     // value-point tile landed
-    auto kfull_bar = [&](int b) { return bar_u32 + 8u * (2 * kRingStages + 7 + b); };     // key-point tiles of pass 1 (two buffers)
+    const uint32_t vfull_bar = bar_u32;                                      // value-point tile landed
+    auto kfull_bar = [&](int b) { return bar_u32 + 8u * (1 + b); };         // key-point tiles of pass 1 (two buffers)
 
     const int N = p.N;
     const int tid = threadIdx.x, lane = tid & 31;
-    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);      // provably warp-uniform: the role branches stay on the uniform datapath
+    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);      // provably warp-uniform
     const int i0 = blockIdx.x * FTI, f = blockIdx.y;
     const long fN = (long)f * N;
     const int ntiles = (N + FTJ - 1) / FTJ;
-    uint32_t tmem_base = 0;
 
-    if (TC) {
-        if (tid == NCOMP) {
-            for (int s = 0; s < kRingStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-            for (int b = 0; b < 2; ++b) { mbar_init(pready_bar(b), 1); mbar_init(pfree_bar(b), 1); }
-            mbar_init(accdone_bar, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        if (warp == NCOMP / 32) {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(512));
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-        }
-        tcgen05_fence_before();
-        __syncthreads();
-        tcgen05_fence_after();
-        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-    }
-
-    if (TC && warp == NCOMP / 32) {
-        // =============================== control warp: V^T ring (TMA) + tcgen05.mma ===============================
-        if (lane == 0) {
-            // instruction descriptor: D = f32, A = B = bf16, A MN-major (V^T from the [j][c] planes), B K-major (P^T), N = 32, M = 128
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | ((uint32_t)(FTI >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const int G = ntiles * 2 * FH;                 // stages: (tile, head, C half)
-            auto issue = [&](int g) {
-                const int s = g % kRingStages;
-                mbar_wait(empty_bar(s), ((g / kRingStages) & 1) ^ 1u);
-                mbar_expect_tx(full_bar(s), kRingStage);
-                const int t = g / (2 * FH), hh = (g % (2 * FH)) >> 1, mh = g & 1;
-                const int c0 = hh * 2 * FC + FC + mh * 128;
-                const uint32_t dst = ring_u32 + s * kRingStage;
-                tma_load_3d(dst, &map_v_hi, full_bar(s), c0, t * FTJ, 0);
-                tma_load_3d(dst + 4096, &map_v_hi, full_bar(s), c0 + 64, t * FTJ, 0);
-                tma_load_3d(dst + 8192, &map_v_lo, full_bar(s), c0, t * FTJ, 0);
-                tma_load_3d(dst + 12288, &map_v_lo, full_bar(s), c0 + 64, t * FTJ, 0);
-            };
-            long long w_full = 0, w_ready = 0, w_empty = 0, t_begin = p.stats ? clock64() : 0;
-            for (int g = 0; g < min(kRingStages - 1, G); ++g) issue(g);
-            for (int g = 0; g < G; ++g) {
-                const int s = g % kRingStages;
-                const int t = g / (2 * FH), rem = g % (2 * FH), hh = rem >> 1, mh = rem & 1;
-                const int par = t & 1;
-                if (rem == 0) {
-                    const long long t0 = p.stats ? clock64() : 0;
-                    mbar_wait(pready_bar(par), (t >> 1) & 1);           // phase A of tile t has written its P^T half
-                    if (p.stats) w_ready += clock64() - t0;
-                    tcgen05_fence_after();
-                }
-                const long long t1 = p.stats ? clock64() : 0;
-                mbar_wait(full_bar(s), (g / kRingStages) & 1);
-                if (p.stats) w_full += clock64() - t1;
-                tcgen05_fence_after();
-                const uint32_t sa = ring_u32 + s * kRingStage;
-                const uint64_t da_hi = make_sw128_mn_desc(sa, 4096), da_lo = make_sw128_mn_desc(sa + 8192, 4096);
-                const uint32_t sb = pb_u32 + hh * 8192 + par * 64;        // this tile's 32 keys = one half of the 128 B rows
-                const uint64_t db_hi = make_sw128_desc(sb), db_lo = make_sw128_desc(sb + 4096);
-                const uint32_t tmem_d = tmem_base + (uint32_t)((hh * 2 + mh) * FTI);
-#pragma unroll
-                for (int ks = 0; ks < ((p.skip & 16) ? 0 : FTJ / 16); ++ks) {
-                    const uint64_t ka = (uint64_t)((2 * 1024) >> 4) * ks;    // MN-major: 16 k rows = 2 swizzle atoms
-                    const uint64_t kb = (uint64_t)(32 >> 4) * ks;            // K-major: 16 elements = 32 B inside the row
-                    umma_bf16(tmem_d, da_lo + ka, db_hi + kb, idesc, (t > 0 || ks > 0) ? 1u : 0u);
-                    umma_bf16(tmem_d, da_hi + ka, db_lo + kb, idesc, 1u);
-                    umma_bf16(tmem_d, da_hi + ka, db_hi + kb, idesc, 1u);
-                }
-                umma_commit(empty_bar(s));
-                if (rem == 2 * FH - 1) {
-                    umma_commit(pfree_bar(par));                          // this P^T half may be overwritten (tile t + 2)
-                    if (t == ntiles - 1) umma_commit(accdone_bar);
-                }
-                if (g + kRingStages - 1 < G) {
-                    const long long t2 = p.stats ? clock64() : 0;
-                    issue(g + kRingStages - 1);
-                    if (p.stats) w_empty += clock64() - t2;
-                }
-            }
-            if (p.stats) {
-                long long* st = p.stats + 16 * ((long)blockIdx.y * gridDim.x + blockIdx.x);
-                st[0] = clock64() - t_begin; st[1] = w_full; st[2] = w_ready; st[3] = w_empty;
-            }
-        }
-    } else {
+    {
         // =============================== compute warps ===============================
         const int h = warp & 7;                                  // phase A / B2: this warp's head
         const int wh = warp >> 3;                                // phase A: row half, B2: key half
@@ -421,25 +272,17 @@ ipa_fused_fwd_kernel(const FusedParams p, const __grid_constant__ CUtensorMap ma
         const int hp = h >> 1, hodd = h & 1;
         const float2* statc = reinterpret_cast<const float2*>(s_stat) + h * FTI + rbase;
         float* sp_w = s_p + rbase * SPS + hp * (2 * FTJ) + lane * 2 + hodd;
-        const bool planes = p.p_hi != nullptr;
         const int nrow_ok = max(0, min(RH, N - i0 - rbase));           // valid rows of this warp's half
-        uint16_t* ph = planes ? p.p_hi + ((long)(f * FH + h) * N + i0 + rbase) * p.ldp : nullptr;
-        uint16_t* pl = planes ? p.p_lo + ((long)(f * FH + h) * N + i0 + rbase) * p.ldp : nullptr;
-        // swizzled bf16 operand tile of this head: row r, key kk -> r*128 + ((kk/8 ^ r%8) << 4) + (kk%8)*2
-        const uint32_t pbh = pb_u32 + h * 8192 + rbase * 128;
+        uint16_t* ph = p.p_hi + ((long)(f * FH + h) * N + i0 + rbase) * p.ldp;
+        uint16_t* pl = p.p_lo + ((long)(f * FH + h) * N + i0 + rbase) * p.ldp;
 
         for (int t = 0; t < ntiles; ++t) {
             const int j0 = t * FTJ;
-            const int par = t & 1;
             // value points of this tile -> s_v[j][h][36]: one TMA box (36 coordinates x 8 heads x 32 residues) of the fp32
             // [F*N][H][60] point tensor; rows past the end of the tensor are zero-filled, rows of the next frame meet p = 0
             if (tid == 0) {
                 mbar_expect_tx(vfull_bar, kSV * 4);
                 tma_load_3d(smem_u32(s_v), &map_pts, vfull_bar, PQ3, 0, (int)(fN + j0));
-            }
-            if (TC && t >= 2) {                                       // the MMAs of tile t - 2 have finished reading this P^T half
-                if (lane == 0) mbar_wait(pfree_bar(par), ((t >> 1) - 1) & 1);
-                __syncwarp();
             }
             // ---- phase A: warp = (head, row half), lane = key ----
             long long tt = timing ? clock64() : 0;
@@ -450,8 +293,6 @@ ipa_fused_fwd_kernel(const FusedParams p, const __grid_constant__ CUtensorMap ma
                 const float mj = jok ? __ldg(mrow + jc) : 0.f;
                 u64 k[12];
                 load_key_global(p.kv_pts, fN, jc, h, k);
-                const uint32_t kk = (uint32_t)(par * FTJ + lane);
-                const uint32_t pb_lane = pbh + ((kk >> 3) << 4) + ((kk & 7) << 1);
 #pragma unroll 1
                 for (int rb = 0; rb < RH; rb += 8) {
                     const float2* rowb = rowc + rb;
@@ -460,7 +301,6 @@ ipa_fused_fwd_kernel(const FusedParams p, const __grid_constant__ CUtensorMap ma
                     float* spb = sp_w + rb * SPS;
                     uint16_t* phb = ph + (long)rb * p.ldp + j;
                     uint16_t* plb = pl + (long)rb * p.ldp + j;
-                    const uint32_t pbb = pb_lane + (uint32_t)(rb * 128);
                     const int nok = nrow_ok - rb;
                     float l0r[8];
 #pragma unroll
@@ -474,28 +314,19 @@ ipa_fused_fwd_kernel(const FusedParams p, const __grid_constant__ CUtensorMap ma
                         float pv = ex2f((s - st.x) * LOG2E) * st.y;      // (s - m) first: exact for the terms that matter
                         pv = jok ? pv : 0.f;
                         spb[rr * SPS] = pv;
-                        if (planes || TC) {
-                            const __nv_bfloat16 bh = __float2bfloat16_rn(pv);
-                            const __nv_bfloat16 bl = __float2bfloat16_rn(pv - __bfloat162float(bh));
-                            if (planes && jok && rr < nok) {
-                                *phb = __bfloat16_as_ushort(bh);
-                                *plb = __bfloat16_as_ushort(bl);
-                            }
-                            phb += p.ldp; plb += p.ldp;
-                            if (TC) {
-                                const uint32_t a = (pbb ^ (uint32_t)(rr << 4)) + (uint32_t)(rr * 128);
-                                asm volatile("st.shared.u16 [%0], %1;" ::"r"(a), "h"(__bfloat16_as_ushort(bh)) : "memory");
-                                asm volatile("st.shared.u16 [%0], %1;" ::"r"(a + 4096u), "h"(__bfloat16_as_ushort(bl)) : "memory");
-                            }
+                        const __nv_bfloat16 bh = __float2bfloat16_rn(pv);
+                        const __nv_bfloat16 bl = __float2bfloat16_rn(pv - __bfloat162float(bh));
+                        if (jok && rr < nok) {
+                            *phb = __bfloat16_as_ushort(bh);
+                            *plb = __bfloat16_as_ushort(bl);
                         }
+                        phb += p.ldp; plb += p.ldp;
                     }
                 }
             }
-            if (TC) fence_proxy_async();                              // generic-proxy stores of P^T -> visible to the tensor core
             if (timing) { const long long n = clock64(); c_a += n - tt; tt = n; }
             comp_sync();
             if (timing) { const long long n = clock64(); c_sync += n - tt; tt = n; }
-            if (TC && tid == 0) mbar_arrive(pready_bar(par));
             // ---- phase B1: pair aggregation, warp = 2 rows, lane = pair channel ----
             if (!(p.skip & 4)) {
                 // eight batches of 8 keys (2 rows x 4 quarters of the tile); the z loads of batch b + 1 are in flight while
@@ -599,28 +430,9 @@ ipa_fused_fwd_kernel(const FusedParams p, const __grid_constant__ CUtensorMap ma
                 }
             }
         }
-        if (TC) {
-            // scalar values O^T[c, i] from TMEM: warp w may read lanes 32 (w % 4) ..; accumulators (h, C half) = w / 4 + 4 k
-            mbar_wait(accdone_bar, 0);
-            tcgen05_fence_after();
-            const int qd = warp & 3;
-#pragma unroll 1
-            for (int kq = 0; kq < 4; ++kq) {
-                const int acc = (warp >> 2) + 4 * kq;
-                uint32_t v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(acc * FTI), v);
-                const int hh = acc >> 1, c = (acc & 1) * 128 + qd * 32 + lane;
-                float* dst = p.cat + (fN + i0) * D + hh * FC + c;
-#pragma unroll
-                for (int r = 0; r < FTI; ++r)
-                    if (i0 + r < N) dst[(long)r * D] = __uint_as_float(v[r]);
-            }
-            tcgen05_fence_before();
-            comp_sync();                                              // pb / ring are free: they become the staging buffer
-        }
         // point features.  The coordinate halves meet in shared memory, s_x[h][row][36]; then thread (h, half, row) transforms
         // points 6 half .. 6 half + 5:  stage[i][0..384) = local xyz + norms, [384..768) = global xyz + norms
-        if (!TC) comp_sync();                                         // (TC: the barrier above) the work buffers are free
+        comp_sync();                                                  // the work buffers are free
         float* s_x = stage + kStage;                                  // 9216 floats behind the staging rows
         {
             u64* dst = reinterpret_cast<u64*>(s_x + (h * FTI + lane) * PV3 + wh * 20);
@@ -675,16 +487,9 @@ ipa_fused_fwd_kernel(const FusedParams p, const __grid_constant__ CUtensorMap ma
             st[4] = clock64() - tc0; st[5] = c_p1; st[6] = c_a; st[7] = c_b1; st[8] = c_b2; st[9] = c_sync; st[10] = c_epi;
         }
     }
-    if (TC) {
-        tcgen05_fence_before();
-        __syncthreads();
-        if (warp == NCOMP / 32) {
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
-        }
-    }
 }
 
-SmemCfg g_fused_cfg[2];
+SmemCfg g_fused_cfg;
 long long* g_ipa_stats = nullptr;      // set by dfold_debug_ipa_stats
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -701,22 +506,6 @@ EncodeTiledFn fused_get_encode() {
     }
     return fn;
 }
-// bf16 plane [rows][ld] viewed as (cols, rows, 1); box = 64 columns x 32 rows, 128B swizzle, out-of-range rows read as zero
-int fused_make_map(CUtensorMap* m, const void* base, long cols, long rows, long ld) {
-    EncodeTiledFn enc = fused_get_encode();
-    DFOLD_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled unavailable (driver too old?)");
-    DFOLD_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && (ld * 2) % 16 == 0, "ipa_fused_fwd: V planes must be 16-byte aligned");
-    cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, 1};
-    cuuint64_t strides[2] = {(cuuint64_t)ld * 2, (cuuint64_t)rows * ld * 2};
-    cuuint32_t box[3] = {64, (cuuint32_t)FTJ, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    DFOLD_REQUIRE(r == CUDA_SUCCESS, "ipa_fused_fwd: cuTensorMapEncodeTiled failed (%d)", (int)r);
-    return 0;
-}
-
 // fp32 point tensor [rows][H][60] viewed as (60, H, rows); box = 36 value coordinates x 8 heads x 32 residues, no swizzle
 int fused_make_pts_map(CUtensorMap* m, const void* base, long rows) {
     EncodeTiledFn enc = fused_get_encode();
@@ -754,31 +543,24 @@ int fused_make_key_map(CUtensorMap* m, const void* base, long rows) {
 using namespace dfold;
 
 // Development aid: when `buf` (device, 16 x int64 per CTA of the next fused-IPA launches) is non-null the kernel records, per
-// CTA, cycle counters of its control thread ({total, wait full, wait P ready, wait empty}) and of compute thread 0
-// ({total, pass 1, phase A, B1, B2, barriers, epilogue}) at slots 0-3 and 4-10.
+// CTA, cycle counters of thread 0 ({total, pass 1, phase A, B1, B2, barriers, epilogue}) at slots 4-10.
 extern "C" int dfold_debug_ipa_stats(long long* buf) {
     g_ipa_stats = buf;
     return 0;
 }
 
-// Fused forward core.  Writes the point and pair columns of the concat buffer and (when p_hi / p_lo are non-null) the
-// bf16 hi/lo probability planes.  With kv_hi / kv_lo (bf16 hi/lo planes of kv [N, H*2C], row stride ldkv, C = 256) the
-// scalar-value columns [0, H*C) are produced in the same kernel on tcgen05 (P stays on the SM); without them they are
-// left to dfold_gemm_bf16x3_batched over the probability planes.
+// Fused forward core.  Writes the point and pair columns of the concat buffer and the bf16 hi/lo probability planes; the
+// scalar-value columns [0, H*C) are left to dfold_gemm_bf16x3_batched over those planes.
 // Shapes: H = 8, Pq = 8, Pv = 12, Cp = 32 (DFOLDv2 preset A); other shapes use dfold_ipa_prob_fwd / dfold_ipa_attn_fwd.
 extern "C" int dfold_ipa_fused_fwd(const float* logit0, const float* q_pts, const float* kv_pts, const float* pair,
                                    const float* quat, const float* trans, const float* mask, const float* gamma,
-                                   uint16_t* p_hi, uint16_t* p_lo, long ldp, const uint16_t* kv_hi, const uint16_t* kv_lo, long ldkv,
+                                   uint16_t* p_hi, uint16_t* p_lo, long ldp,
                                    int F, int N, int H, int C, int Pq, int Pv, int Cp,
                                    int dfold, float inf, float eps, float* out_cat, void* stream) {
     DFOLD_REQUIRE(F > 0 && N > 0, "ipa_fused_fwd: empty problem");
     DFOLD_REQUIRE(H == FH && Pq == FPQ && Pv == FPV && Cp == FCP, "ipa_fused_fwd: built for H=8, Pq=8, Pv=12, Cp=32 (got %d, %d, %d, %d)", H, Pq, Pv, Cp);
-    DFOLD_REQUIRE((p_hi == nullptr) == (p_lo == nullptr) && (!p_hi || ldp >= N), "ipa_fused_fwd: bad probability planes");
-    DFOLD_REQUIRE((kv_hi == nullptr) == (kv_lo == nullptr), "ipa_fused_fwd: bad V planes");
+    DFOLD_REQUIRE(p_hi != nullptr && p_lo != nullptr && ldp >= N, "ipa_fused_fwd: bad probability planes");
     DFOLD_REQUIRE(F <= 65535 && (long)N * N < (1l << 31), "ipa_fused_fwd: problem too large for one launch");
-    const bool tc = kv_hi != nullptr;
-    DFOLD_REQUIRE(tc || p_hi, "ipa_fused_fwd: without V planes the probability planes are required (O = P V runs on the GEMM)");
-    DFOLD_REQUIRE(!tc || (C == FC && ldkv >= (long)H * 2 * C), "ipa_fused_fwd: the tensor-core variant needs C = 256");
     FusedParams p;
     p.logit0 = logit0; p.q_pts = q_pts; p.kv_pts = kv_pts; p.pair = pair; p.quat = quat; p.trans = trans; p.mask = mask;
     p.gamma = gamma; p.p_hi = p_hi; p.p_lo = p_lo; p.ldp = ldp; p.cat = out_cat; p.F = F; p.N = N; p.C = C; p.dfold = dfold;
@@ -786,18 +568,11 @@ extern "C" int dfold_ipa_fused_fwd(const float* logit0, const float* q_pts, cons
     { const char* e = getenv("DFOLD_IPA_DEBUG_SKIP"); p.skip = e ? atoi(e) : 0; }
     p.stats = g_ipa_stats;
     dim3 grid((unsigned)cdiv(N, FTI), (unsigned)F);
-    CUtensorMap maps[4];
+    CUtensorMap maps[2];
     memset(maps, 0, sizeof(maps));
-    if (fused_make_pts_map(&maps[2], kv_pts, (long)F * N)) return 1;
-    if (fused_make_key_map(&maps[3], kv_pts, (long)F * N)) return 1;
-    if (tc) {
-        if (fused_make_map(&maps[0], kv_hi, (long)H * 2 * C, N, ldkv)) return 1;
-        if (fused_make_map(&maps[1], kv_lo, (long)H * 2 * C, N, ldkv)) return 1;
-        if (ensure_dyn_smem(ipa_fused_fwd_kernel<true>, FCfg<true>::kBytes, g_fused_cfg[1], "ipa_fused_fwd")) return 1;
-        ipa_fused_fwd_kernel<true><<<grid, FCfg<true>::kThreads, FCfg<true>::kBytes, as_stream(stream)>>>(p, maps[0], maps[1], maps[2], maps[3]);
-    } else {
-        if (ensure_dyn_smem(ipa_fused_fwd_kernel<false>, FCfg<false>::kBytes, g_fused_cfg[0], "ipa_fused_fwd")) return 1;
-        ipa_fused_fwd_kernel<false><<<grid, FCfg<false>::kThreads, FCfg<false>::kBytes, as_stream(stream)>>>(p, maps[0], maps[1], maps[2], maps[3]);
-    }
+    if (fused_make_pts_map(&maps[0], kv_pts, (long)F * N)) return 1;
+    if (fused_make_key_map(&maps[1], kv_pts, (long)F * N)) return 1;
+    if (ensure_dyn_smem(ipa_fused_fwd_kernel, kFusedBytes, g_fused_cfg, "ipa_fused_fwd")) return 1;
+    ipa_fused_fwd_kernel<<<grid, NCOMP, kFusedBytes, as_stream(stream)>>>(p, maps[0], maps[1]);
     return check_launch("ipa_fused_fwd_kernel");
 }

@@ -1,9 +1,9 @@
 // Invariant point attention, second-generation decomposition for the tensor-core path.
 //
 // The attention probabilities are materialised ONCE as bf16 hi/lo planes  P[F,H,N,N8]  (same bytes as fp32) and
-// every dense contraction over them runs on the tcgen05 split-bf16 GEMM (csrc/gemm_sm100.cu):
+// every dense contraction over them runs on the wgmma split-bf16 GEMM (csrc/gemm_sm90.cu):
 //     forward : O = P V                       (batched K-major GEMM, written straight into the concat buffer)
-//     backward: dP = dO V^T, dV = P^T dO (split-K), dV_pts = P^T dO_pts, dZ = sum_{f,h} P dO_pair
+//     backward: dP = dO V^T, dV = P^T dO, dV_pts = P^T dO_pts, dZ = sum_{f,h} P dO_pair
 // The kernels here do the part that is NOT a GEMM and must stay exact fp32 on coordinate differences:
 //   ipa_prob_fwd   logits = logit0 - gamma/2 * sum_p |q_p - k_p|^2 + mask, exact row softmax (whole rows live in shared
 //                  memory), P planes, aggregated global value points, local-frame transform, norms
@@ -324,18 +324,27 @@ __global__ void __launch_bounds__(256) ipa_ds_kernel(const V2Params p, const flo
     if (tid == 0) {
         float t = 0.f;
         for (int w = 0; w < 8; ++w) t += s_red[w];
-        atomicAdd(dgamma + h, t);
+        dgamma[(long)h * p.F * p.N + (long)blockIdx.z * gridDim.x + blockIdx.x] = t;   // per-CTA partial (no atomics)
     }
     (void)gam;
 }
 
 // Second-generation dS kernel (Pq = 8): the value-point term d_og.v_pts arrives precomputed from the tensor cores (Tog,
 // [F,H,N,N]), each lane keeps its key's 24 coordinates in registers, the query points are broadcast 16 bytes at a time and
-// the squared distance for d(gamma) runs on packed FADD2 / FFMA2 -- 6 shared-memory loads per pair instead of ~120.
+// the squared distance for d(gamma) runs on coordinate pairs held as 64-bit words -- 6 shared-memory loads per pair
+// instead of ~120.  sm_90 has no packed FP32 arithmetic: each pair op is two scalar round-to-nearest ops.
 // grid (ceil(N/32), H, F), 256 threads: 4 rows per warp, keys across lanes.
 typedef unsigned long long u64v2;
-__device__ __forceinline__ u64v2 v2_sub2(u64v2 a, u64v2 b) { u64v2 r; asm("sub.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ u64v2 v2_fma2(u64v2 a, u64v2 b, u64v2 c) { u64v2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
+__device__ __forceinline__ u64v2 v2_sub2(u64v2 a, u64v2 b) {
+    const float2 x = *reinterpret_cast<const float2*>(&a), y = *reinterpret_cast<const float2*>(&b);
+    const float2 r = make_float2(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y));
+    return *reinterpret_cast<const u64v2*>(&r);
+}
+__device__ __forceinline__ u64v2 v2_fma2(u64v2 a, u64v2 b, u64v2 c) {
+    const float2 x = *reinterpret_cast<const float2*>(&a), y = *reinterpret_cast<const float2*>(&b), z = *reinterpret_cast<const float2*>(&c);
+    const float2 r = make_float2(__fmaf_rn(x.x, y.x, z.x), __fmaf_rn(x.y, y.y, z.y));
+    return *reinterpret_cast<const u64v2*>(&r);
+}
 __global__ void __launch_bounds__(256) ipa_ds2_kernel(const V2Params p, const float* __restrict__ delta, const float* __restrict__ dPg,
                                                       const float* __restrict__ Tz, const float* __restrict__ Tog,
                                                       float* __restrict__ dS, float* __restrict__ dgamma) {
@@ -407,7 +416,7 @@ __global__ void __launch_bounds__(256) ipa_ds2_kernel(const V2Params p, const fl
     if (tid == 0) {
         float t = 0.f;
         for (int w = 0; w < 8; ++w) t += s_red[w];
-        atomicAdd(dgamma + h, t);
+        dgamma[(long)h * p.F * p.N + (long)blockIdx.z * gridDim.x + blockIdx.x] = t;   // per-CTA partial (no atomics)
     }
 }
 

@@ -34,17 +34,14 @@ __device__ __forceinline__ uint32_t split_pack(float x) {
 }
 
 // x[R, C] (row stride ld) -> hi/lo [R, ldo] and optionally transposed hi_t/lo_t [C, ldt].
-// Optional: relu on the input, a gate (x *= gate > 0), column sums of the (gated) input.
+// Optional: relu on the input, a gate (x *= gate > 0).  The column sums of the (gated) input come from colsum_kernel.
 __global__ void split2d_kernel(const float* __restrict__ x, long R, long C, long ld, int pre_relu,
                                const float* __restrict__ gate, long ldg,
                                uint16_t* __restrict__ hi, uint16_t* __restrict__ lo, long ldo, long cpad,
-                               uint16_t* __restrict__ hit, uint16_t* __restrict__ lot, long ldt, long rpad,
-                               float* __restrict__ colsum) {
+                               uint16_t* __restrict__ hit, uint16_t* __restrict__ lot, long ldt, long rpad) {
     __shared__ uint32_t tile[32][33];
-    __shared__ float csum[8][33];
     const long r0 = (long)blockIdx.y * 32, c0 = (long)blockIdx.x * 32;
     const int tx = threadIdx.x, ty = threadIdx.y;       // 32 x 8
-    float part = 0.f;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const long r = r0 + ty + i * 8, c = c0 + tx;
@@ -54,7 +51,6 @@ __global__ void split2d_kernel(const float* __restrict__ x, long R, long C, long
             if (pre_relu) v = fmaxf(v, 0.f);
             if (gate) v = (gate[r * ldg + c] > 0.f) ? v : 0.f;
         }
-        part += v;
         const uint32_t pk = split_pack(v);
         tile[ty + i * 8][tx] = pk;
         if (hi && r < R && c < cpad) {      // columns in [C, cpad) are written as zero padding
@@ -62,16 +58,7 @@ __global__ void split2d_kernel(const float* __restrict__ x, long R, long C, long
             lo[r * ldo + c] = (uint16_t)(pk & 0xffffu);
         }
     }
-    if (colsum) {
-        csum[ty][tx] = part;
-    }
     __syncthreads();
-    if (colsum && ty == 0) {
-        float s = 0.f;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) s += csum[i][tx];
-        if (c0 + tx < C) atomicAdd(colsum + c0 + tx, s);
-    }
     if (hit) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -392,6 +379,59 @@ __global__ void gln_bwd_apply_kernel(const float* __restrict__ x, const float* _
 // ---------------------------------------------------------------------------------------------------
 // per-row LayerNorm with affine (nn.LayerNorm / openfold LayerNorm), one warp per row
 // ---------------------------------------------------------------------------------------------------
+// Column sums over all rows in one fixed order (no atomics, so the result is the same from run to run): one CTA per 32
+// columns, 32 row lanes; lane r adds rows r, r + 32, ... in turn, then the 32 lane sums are added in lane order.
+__global__ void __launch_bounds__(1024) colsum_kernel(const float* __restrict__ x, long R, long C, long ld, int pre_relu,
+                                                      const float* __restrict__ gate, long ldg, float* __restrict__ colsum) {
+    __shared__ float red[32][33];
+    const int tx = threadIdx.x, ty = threadIdx.y;
+    const long c = (long)blockIdx.x * 32 + tx;
+    float s = 0.f;
+    if (c < C) {
+        for (long r = ty; r < R; r += 32) {
+            float v = x[r * ld + c];
+            if (pre_relu) v = fmaxf(v, 0.f);
+            if (gate) v = (gate[r * ldg + c] > 0.f) ? v : 0.f;
+            s += v;
+        }
+    }
+    red[ty][tx] = s;
+    __syncthreads();
+    if (ty == 0 && c < C) {
+        float t = 0.f;
+        for (int i = 0; i < 32; ++i) t += red[i][tx];
+        colsum[c] += t;
+    }
+}
+
+// LayerNorm weight / bias gradients dw[c] += sum_r dy[r][c] xhat[r][c], db[c] += sum_r dy[r][c], in the fixed order of
+// colsum_kernel.
+__global__ void __launch_bounds__(1024) row_ln_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dy,
+                                                            const float* __restrict__ stats, float* __restrict__ dw,
+                                                            float* __restrict__ db, long rows, int C) {
+    __shared__ float red_w[32][33], red_b[32][33];
+    const int tx = threadIdx.x, ty = threadIdx.y;
+    const long c = (long)blockIdx.x * 32 + tx;
+    float sw = 0.f, sb = 0.f;
+    if (c < C) {
+        for (long r = ty; r < rows; r += 32) {
+            const float g = dy[r * C + c];
+            const float xh = (x[r * C + c] - stats[2 * r]) * stats[2 * r + 1];
+            sw += g * xh;
+            sb += g;
+        }
+    }
+    red_w[ty][tx] = sw;
+    red_b[ty][tx] = sb;
+    __syncthreads();
+    if (ty == 0 && c < C) {
+        float tw = 0.f, tb = 0.f;
+        for (int i = 0; i < 32; ++i) { tw += red_w[i][tx]; tb += red_b[i][tx]; }
+        dw[c] += tw;
+        db[c] += tb;
+    }
+}
+
 __global__ void row_ln_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
                                   float* __restrict__ y, float* __restrict__ stats, long rows, int C, float eps) {
     const long row = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -425,8 +465,6 @@ __global__ void row_ln_bwd_kernel(const float* __restrict__ x, const float* __re
     for (int c = lane; c < C; c += 32) {
         const float xh = (xr[c] - mean) * rstd, g = gr[c] * w[c];
         dx[row * C + c] = rstd * (g - s1 - xh * s2);
-        atomicAdd(dw + c, gr[c] * xh);
-        atomicAdd(db + c, gr[c]);
     }
 }
 
@@ -436,7 +474,7 @@ __global__ void row_ln_bwd_kernel(const float* __restrict__ x, const float* __re
 using namespace dfold;
 
 extern "C" const char* dfold_last_error(void) { return g_err; }
-extern "C" int dfold_abi_version(void) { return 2; }
+extern "C" int dfold_abi_version(void) { return 3; }
 
 // id of the CUDA-graph capture `stream` is recording into (0 when the stream is not capturing).  The host side keys
 // its cached operand planes on it: planes built inside one capture must never be reused by another graph.
@@ -461,7 +499,11 @@ extern "C" int dfold_split2d(const float* x, long R, long C, long ld, int pre_re
     // the grid covers the padded extents so the padding columns/rows are written as zeros
     const long cols = (hi && cpad > C) ? cpad : C;
     const long rows = (hi_t && rpad > R) ? rpad : R;
-    if (hi && !hi_t && !colsum && (ld & 3) == 0 && (ldo & 3) == 0 && (cpad & 3) == 0 && (!gate || (ldg & 3) == 0) &&
+    if (colsum) {
+        colsum_kernel<<<(unsigned)cdiv(C, 32), dim3(32, 32), 0, as_stream(stream)>>>(x, R, C, ld, pre_relu, gate, ldg, colsum);
+        if (check_launch("colsum_kernel")) return 1;
+    }
+    if (hi && !hi_t && (ld & 3) == 0 && (ldo & 3) == 0 && (cpad & 3) == 0 && (!gate || (ldg & 3) == 0) &&
         ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(gate)) & 15) == 0 &&
         ((reinterpret_cast<uintptr_t>(hi) | reinterpret_cast<uintptr_t>(lo)) & 7) == 0) {
         const long c4n = cpad / 4, n = R * c4n;
@@ -469,7 +511,7 @@ extern "C" int dfold_split2d(const float* x, long R, long C, long ld, int pre_re
         return check_launch("split2d_vec_kernel");
     }
     dim3 grid((unsigned)cdiv(cols, 32), (unsigned)cdiv(rows, 32));
-    split2d_kernel<<<grid, dim3(32, 8), 0, as_stream(stream)>>>(x, R, C, ld, pre_relu, gate, ldg, hi, lo, ldo, cpad, hi_t, lo_t, ldt, rpad, colsum);
+    split2d_kernel<<<grid, dim3(32, 8), 0, as_stream(stream)>>>(x, R, C, ld, pre_relu, gate, ldg, hi, lo, ldo, cpad, hi_t, lo_t, ldt, rpad);
     return check_launch("split2d_kernel");
 }
 
@@ -493,8 +535,8 @@ extern "C" int dfold_taps_to_param(const float* g, int O, int I, int T, float* o
 }
 
 // Strides are in elements: *_rs row, *_cs column, *_bs / *_bs2 outer / inner batch.  C = act(alpha*A.B^T + bias) + beta*R.
-// ksplit > 1 splits the K range over extra CTAs (tiny-output weight gradients with K = all pixels) and atomically
-// accumulates into a zeroed C.
+// ksplit > 1 splits the K range over extra CTAs and atomically accumulates into a zeroed C (the summation order, and with
+// it the last bits, then varies from run to run; the package's own callers split K with batched partials instead).
 extern "C" int dfold_sgemm(const float* A, long a_rs, long a_cs, long a_bs, long a_bs2,
                            const float* B, long b_rs, long b_cs, long b_bs, long b_bs2,
                            float* C, long c_rs, long c_cs, long c_bs, long c_bs2,
@@ -542,7 +584,9 @@ extern "C" int dfold_row_layernorm_bwd(const float* x, const float* w, const flo
                                        long rows, int C, void* stream) {
     DFOLD_REQUIRE(rows > 0 && C > 0, "dfold_row_layernorm_bwd: empty input");
     row_ln_bwd_kernel<<<(unsigned)cdiv(rows, 8), 256, 0, as_stream(stream)>>>(x, w, dy, stats, dx, dw, db, rows, C);
-    return check_launch("row_ln_bwd_kernel");
+    if (check_launch("row_ln_bwd_kernel")) return 1;
+    row_ln_wgrad_kernel<<<(unsigned)cdiv(C, 32), dim3(32, 32), 0, as_stream(stream)>>>(x, dy, stats, dw, db, rows, C);
+    return check_launch("row_ln_wgrad_kernel");
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -591,7 +635,11 @@ extern "C" int dfold_adam_amsgrad(float* param, const float* grad, float* exp_av
     cudaStream_t st = dfold::as_stream(stream);
     if (tick) dfold::adam_tick_kernel<<<1, 1, 0, st>>>(step);      // chunked callers advance the step once per optimizer step
     const long n4 = n / 4;
-    const int blocks = (int)(dfold::cdiv(n4, 256) < 148 * 16 ? dfold::cdiv(n4, 256) : 148 * 16);
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
+        sms = 132;
+    const long cap = 16L * sms;                                     // 16 CTAs of 256 threads per SM, grid-stride beyond
+    const int blocks = (int)(dfold::cdiv(n4, 256) < cap ? dfold::cdiv(n4, 256) : cap);
     dfold::adam_amsgrad_kernel<<<blocks, 256, 0, st>>>(param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n4, step, lr, beta1, beta2, eps, grad_scale);
     return dfold::check_launch("adam_amsgrad_kernel");
 }

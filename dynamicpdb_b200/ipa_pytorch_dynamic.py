@@ -2,10 +2,10 @@
 
 Same class names, constructor arguments, forward signatures and ``state_dict`` layout as the reference, so the
 reference's ``train_DFOLD_dynamics.py`` / ``eval_DFOLD_dynamics.py`` run unchanged against it (through the import
-overlay in ``overlay/``).  All arithmetic is dispatched to the hand-written sm_100a kernels in ``csrc/`` through
+overlay in ``overlay/``).  All arithmetic is dispatched to the hand-written sm_90a kernels in ``csrc/`` through
 ``kernels`` (C-ABI, ctypes); there is no CPU fallback — the ops raise if the extension or a CUDA device is missing.
 
-B200-first restructuring that keeps results identical to the reference:
+GPU-first restructuring that keeps results identical to the reference:
   * activations stay channels-last ``[frames, residues, C]`` end to end — the reference permutes to NCHW for its
     ``Conv2d`` stack (ipa_pytorch_dynamic.py:694); here the 5x5 frame x residue convolution is an implicit GEMM
     over TMA halo tiles of the channels-last tensor;

@@ -1,6 +1,6 @@
 """Autograd-aware operator surface over the C-ABI library ``libdfold_b200.so`` (include/dfold_b200.h).
 
-Every function here launches hand-written sm_100a kernels through ctypes with raw device pointers and the
+Every function here launches hand-written sm_90a kernels through ctypes with raw device pointers and the
 current CUDA stream.  There is NO CPU path and no fallback to torch library kernels for the arithmetic: if the
 shared library is missing, or a tensor is not on a CUDA device, the ops raise.  (The tests exercise the host-side
 module logic on CPU by monkey-patching these names with the oracle — that seam lives in tests/, not here.)
@@ -48,10 +48,10 @@ _SIGS = {
     "dfold_ipa_pre_bwd": "pp" + "iiiiiii" + "pp" + "pppp" + "p",
     "dfold_ipa_prob_fwd": "plppplpppp" + "ppl" + "iiiiiiii" + "ff" + "pp",
     "dfold_ipa_pair_fwd": "plppplpppp" + "ppl" + "iiiiiiii" + "ff" + "pp",
-    "dfold_ipa_fused_fwd": "pppppppp" + "ppl" + "ppl" + "iiiiiiii" + "ff" + "pp",
+    "dfold_ipa_fused_fwd": "pppppppp" + "ppl" + "iiiiiiii" + "ff" + "pp",
     "dfold_ipa_ds_bwd": "plppplpppp" + "ppl" + "iiiiiiii" + "ff" + "pppppp" + "pppp" + "p",
     "dfold_gemm_bf16x3_batched": "ppllll" + "liill" + "ppllll" + "llil" + "pllilf" + "p",
-    "dfold_gemm_wgrad_bf16x3_batched": "pplllll" + "pplllll" + "lll" + "ii" + "iiiil" + "pllf" + "p",
+    "dfold_gemm_wgrad_bf16x3_batched": "pplllll" + "pplllll" + "lll" + "i" + "iiiil" + "pllf" + "p",
     "dfold_score_fwd": "ppppp" + "pidddd" + "ffpil" + "ppi" + "p",
     "dfold_score_bwd": "ppppp" + "pidddd" + "ffpil" + "ppi" + "pp" + "p",
     "dfold_frames_to_atoms_fwd": "pippp" + "pppppp" + "ppp" + "lp",
@@ -73,7 +73,7 @@ def lib():
     if _LIB is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
-                f"{LIB_PATH} not found: build the sm_100a extension first (python -m dynamicpdb_b200.build or "
+                f"{LIB_PATH} not found: build the sm_90a extension first (python -m dynamicpdb_b200.build or "
                 "__graft_entry__.build()).  dynamicpdb_b200 has no CPU / PyTorch fallback.")
         L = ctypes.CDLL(LIB_PATH)
         for name, sig in _SIGS.items():
@@ -139,6 +139,19 @@ def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+_SMS = {}
+
+
+def _sm_count(dev) -> int:
+    """Streaming multiprocessors of `dev` (132 on an H100 SXM)."""
+    idx = torch.device(dev).index
+    if idx is None:
+        idx = torch.cuda.current_device()
+    if idx not in _SMS:
+        _SMS[idx] = torch.cuda.get_device_properties(idx).multi_processor_count
+    return _SMS[idx]
+
+
 def _on_device(fn):
     """Run an autograd Function's forward / backward with the CUDA device of its tensors current.  The C-ABI launches,
     cuTensorMapEncode and the stream lookup all act on the CURRENT device, and the reference trainer's single-GPU
@@ -162,7 +175,7 @@ def _on_device(fn):
 def _need_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("dynamicpdb_b200 ops need CUDA tensors (B200 / sm_100a); there is no CPU fallback")
+            raise RuntimeError("dynamicpdb_b200 ops need CUDA tensors (H100 / sm_90a); there is no CPU fallback")
 
 
 def _f32c(t: torch.Tensor) -> torch.Tensor:
@@ -180,15 +193,16 @@ def _pad8(n: int) -> int:
 # --------------------------------------------------------------------------------------------------
 def _sgemm(A, a_off, a_rs, a_cs, a_bs, a_bs2, B, b_off, b_rs, b_cs, b_bs, b_bs2, C, c_off, c_rs, c_cs, c_bs, c_bs2,
            M, N, K, *, R=None, r_off=0, r_rs=0, r_cs=0, r_bs=0, r_bs2=0, bias=None, batch=1, batch2=1,
-           alpha=1.0, beta=1.0, act=0, pre_relu=0, ksplit=1):
+           alpha=1.0, beta=1.0, act=0, pre_relu=0):
     _check(lib().dfold_sgemm(_ptr(A, a_off), a_rs, a_cs, a_bs, a_bs2, _ptr(B, b_off), b_rs, b_cs, b_bs, b_bs2,
                              _ptr(C, c_off), c_rs, c_cs, c_bs, c_bs2, _ptr(R, r_off), r_rs, r_cs, r_bs, r_bs2,
-                             _ptr(bias), batch, batch2, M, N, K, alpha, beta, act, pre_relu, ksplit, _stream()), "dfold_sgemm")
+                             _ptr(bias), batch, batch2, M, N, K, alpha, beta, act, pre_relu, 1, _stream()), "dfold_sgemm")
 
 
 def _split2d(x2: torch.Tensor, *, pre_relu=False, gate=None, want=True, want_t=False, colsum=None,
              t_out=None, t_ld=None, t_off=0, rpad=None):
-    """x2 [R, C] fp32 contiguous -> (hi, lo) [R, C8] and / or transposed planes [C, R8] (or into ``t_out``)."""
+    """x2 [R, C] fp32 contiguous -> (hi, lo) [R, C8] and / or transposed planes [C, R8] (or into ``t_out``); ``colsum``
+    ([C], zeroed) receives the column sums of the gated input."""
     R, C = x2.shape
     hi = lo = hit = lot = None
     c8 = _pad8(C)
@@ -311,7 +325,7 @@ _ACT = {None: 0, "relu": 1}
 
 
 def _use_tensor_cores(M: int, N: int, K: int) -> bool:
-    # the 128 x BN tcgen05 tile needs 16-byte aligned K rows; tiny problems stay on the SIMT kernel
+    # the 128 x BN wgmma tile needs 16-byte aligned K rows; tiny problems stay on the SIMT kernel
     return K % 8 == 0 and K >= 64 and N >= 16 and M >= 32 and (M * N * K) >= (1 << 18)
 
 
@@ -382,9 +396,16 @@ class _LinearFn(Function):
                 xr = torch.relu(x2) if pre_relu else x2
                 # tiny [N, K] output reduced over all M rows: split the reduction over CTAs
                 tiles = ((N_ + 63) // 64) * ((K_ + 63) // 64)
-                ks = max(1, min(M_ // 512, 592 // tiles, 256))
-                dw = (torch.zeros if ks > 1 else torch.empty)((N_, K_), dtype=torch.float32, device=g.device)
-                _sgemm(g, 0, 1, N_, 0, 0, xr, 0, 1, K_, 0, 0, dw, 0, K_, 1, 0, 0, N_, K_, M_, ksplit=ks)
+                ks = max(1, min(M_ // 512, 4 * _sm_count(g.device) // tiles, 256))
+                # chunks of `kc` rows as a batch of partial products [ks (+1 for the tail), N, K], added in a fixed order
+                # (split-K with atomics would make the last bits vary from run to run)
+                kc = M_ // ks
+                tail = M_ - ks * kc
+                part = torch.empty((ks + (1 if tail else 0), N_, K_), dtype=torch.float32, device=g.device)
+                _sgemm(g, 0, 1, N_, kc * N_, 0, xr, 0, 1, K_, kc * K_, 0, part, 0, K_, 1, N_ * K_, 0, N_, K_, kc, batch=ks)
+                if tail:
+                    _sgemm(g, ks * kc * N_, 1, N_, 0, 0, xr, ks * kc * K_, 1, K_, 0, 0, part, ks * N_ * K_, K_, 1, 0, 0, N_, K_, tail)
+                dw = part.sum(0) if part.shape[0] > 1 else part[0]
             if need_b:
                 db = g.sum(0)
         if dx is not None:
@@ -787,11 +808,12 @@ class _IpaAttnFn(Function):
         Pm, dS = new(H_, F_, N_, N_), new(H_, F_, N_, N_)
         dq_pts, dkv_pts = new(*q_pts.shape), new(*kv_pts.shape)
         dquat, dtrans = new(*quat.shape), new(*trans.shape)
-        dgamma = torch.zeros(H_, dtype=torch.float32, device=dev)
+        dgamma_part = torch.zeros(H_, F_ * N_, dtype=torch.float32, device=dev)      # per-CTA partials, summed in order
         args = _IpaAttnFn._args(logit0, kv, q_pts, kv_pts, pair, quat, trans, mask, gamma, F_, N_, H_, C_, Pq, Pv, Cp, dfold, inf, eps)
         _check(lib().dfold_ipa_attn_bwd(*args, _ptr(cat), _ptr(lse), _ptr(dcat), _ptr(d_og), _ptr(delta), _ptr(Pm), _ptr(dS),
-                                        _ptr(dq_pts), _ptr(dkv_pts), _ptr(dquat), _ptr(dtrans), _ptr(dgamma), _stream()),
+                                        _ptr(dq_pts), _ptr(dkv_pts), _ptr(dquat), _ptr(dtrans), _ptr(dgamma_part), _stream()),
                "dfold_ipa_attn_bwd")
+        dgamma = dgamma_part.sum(1)
         NN = N_ * N_
         # ---- value gradient  dv[j,h,c] = sum_{f,i} P[h,f,i,j] dO[f,i,h,c] ----
         Fs = kv.shape[0]
@@ -857,38 +879,29 @@ class _IpaAttnTCFn(Function):
         n8 = _pad8(N_)
         cat = torch.empty((F_, N_, D), dtype=torch.float32, device=dev)
         fused = _fused_fwd_ok(H_, Pq, Pv, Cp)
-        fused_tc = fused and C_ == 256 and os.environ.get("DFOLD_IPA_FUSED_TC", "1") != "0"
-        # the probability planes feed the backward GEMMs (and the separate P V GEMM when the forward is not fully fused)
-        need_planes = (not fused_tc) or any(ctx.needs_input_grad)
-        p_hi = torch.empty((F_, H_, N_, n8), dtype=torch.int16, device=dev) if need_planes else None
-        p_lo = torch.empty((F_, H_, N_, n8), dtype=torch.int16, device=dev) if need_planes else None
+        # the probability planes feed the P V GEMM and the backward GEMMs
+        p_hi = torch.empty((F_, H_, N_, n8), dtype=torch.int16, device=dev)
+        p_lo = torch.empty((F_, H_, N_, n8), dtype=torch.int16, device=dev)
         args = _IpaAttnTCFn._v2args(logit0, q_pts, kv_pts, pair, quat, trans, mask, gamma, p_hi, p_lo, n8, F_, N_, H_, C_, Pq, Pv, Cp, dfold, inf, eps)
         alg_bytes = 4.0 * (F_ * N_ * (H_ * (4 * C_ + 3 * (2 * Pq + Pv) + 8 * Pv + Cp) + 8) + N_ * N_ * (H_ + Cp))
-        kv_hi = kv_lo = None
         with _timed("ipa_fwd", alg_bytes):
             if fused:
-                # one kernel: distances, exact softmax, pair + value-point aggregation, frame transform, P planes and
-                # (fused_tc) O = P V on tcgen05 straight from the shared-memory P tile
-                if fused_tc:
-                    kv_hi, kv_lo = _planes_rows(kv.reshape(N_, H_ * 2 * C_))                # [N, H*2C] bf16 hi / lo
+                # one kernel: distances, exact softmax, pair + value-point aggregation, frame transform, P planes
                 _check(lib().dfold_ipa_fused_fwd(_ptr(logit0), _ptr(q_pts), _ptr(kv_pts), _ptr(pair), _ptr(quat), _ptr(trans),
                                                  _ptr(mask), _ptr(gamma), _ptr(p_hi), _ptr(p_lo), n8,
-                                                 _ptr(kv_hi), _ptr(kv_lo), 0 if kv_hi is None else kv_hi.shape[1],
                                                  F_, N_, H_, C_, Pq, Pv, Cp, int(dfold), inf, eps, _ptr(cat), _stream()),
                        "dfold_ipa_fused_fwd")
             else:
                 _check(lib().dfold_ipa_prob_fwd(*args, _ptr(cat), _stream()), "dfold_ipa_prob_fwd")
-            if not fused_tc:
-                # O = P V  on the tensor cores, written into the o-columns of the concat buffer
-                vt = kv[0, :, :, C_:].permute(1, 2, 0).reshape(H_ * C_, N_).contiguous()        # [H*C, N]
-                vt_hi, vt_lo = _planes_rows(vt)
-                _check(lib().dfold_gemm_bf16x3_batched(
-                    _ptr(p_hi), _ptr(p_lo), F_ * H_, N_, N_, n8, F_ * H_, H_, 1, 0, N_,
-                    _ptr(vt_hi), _ptr(vt_lo), H_, C_, N_, vt_hi.shape[1], 0, 0, 1, C_,
-                    _ptr(cat), D, F_ * N_, H_, C_, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
+            # O = P V  on the tensor cores, written into the o-columns of the concat buffer
+            vt = kv[0, :, :, C_:].permute(1, 2, 0).reshape(H_ * C_, N_).contiguous()        # [H*C, N]
+            vt_hi, vt_lo = _planes_rows(vt)
+            _check(lib().dfold_gemm_bf16x3_batched(
+                _ptr(p_hi), _ptr(p_lo), F_ * H_, N_, N_, n8, F_ * H_, H_, 1, 0, N_,
+                _ptr(vt_hi), _ptr(vt_lo), H_, C_, N_, vt_hi.shape[1], 0, 0, 1, C_,
+                _ptr(cat), D, F_ * N_, H_, C_, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
             if not fused:
                 _check(lib().dfold_ipa_pair_fwd(*args, _ptr(cat), _stream()), "dfold_ipa_pair_fwd")
-        ctx.kv_planes = (kv_hi, kv_lo)
         ctx.save_for_backward(logit0, kv, q_pts, kv_pts, pair, quat, trans, mask, gamma, cat, p_hi, p_lo)
         ctx.meta = (Pq, Pv, dfold, inf, eps)
         return cat
@@ -914,9 +927,7 @@ class _IpaAttnTCFn(Function):
                                        _ptr(d_og), _ptr(delta), _ptr(dquat), _ptr(dtrans), _stream()), "dfold_ipa_pre_bwd")
         # ---- dP = dO V^T  (batched over (f, h); K = the head's C columns of dO) ----
         dc_hi, dc_lo = _planes_rows(dcat.reshape(F_ * N_, D))                       # [F*N, D8]
-        kv_hi, kv_lo = ctx.kv_planes
-        if kv_hi is None:
-            kv_hi, kv_lo = _planes_rows(kv.reshape(N_, H_ * 2 * C_))                # [N, H*2C]
+        kv_hi, kv_lo = _planes_rows(kv.reshape(N_, H_ * 2 * C_))                    # [N, H*2C]
         dP = new(F_, H_, N_, N_)
         _check(lib().dfold_gemm_bf16x3_batched(
             _ptr(dc_hi), _ptr(dc_lo), F_, N_, D, dc_hi.shape[1], F_ * H_, H_, H_, C_, C_,
@@ -934,7 +945,7 @@ class _IpaAttnTCFn(Function):
             _ptr(Tz), N_, N_ * F_ * H_, 1, 0, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
         # ---- dS, d(gamma), point gradients ----
         dS = new(F_, H_, N_, N_)
-        dgamma = torch.zeros(H_, dtype=torch.float32, device=dev)
+        dgamma_part = torch.zeros(H_, F_ * N_, dtype=torch.float32, device=dev)      # per-CTA partials, summed in order
         dq_pts, dkv_pts = new(*q_pts.shape), new(*kv_pts.shape)
         args = _IpaAttnTCFn._v2args(logit0, q_pts, kv_pts, pair, quat, trans, mask, gamma, p_hi, p_lo, n8, F_, N_, H_, C_, Pq, Pv, Cp, dfold, inf, eps)
         pts_gemm = PQ3 <= 31 and os.environ.get("DFOLD_IPA_PTS_GEMM", "1") != "0"
@@ -951,8 +962,9 @@ class _IpaAttnTCFn(Function):
                 _ptr(dg_hi), _ptr(dg_lo), F_ * H_, N_, PV3, dg_hi.shape[1], F_ * H_, F_ * H_, 1, 0, PV3,
                 _ptr(vp_hi), _ptr(vp_lo), F_ * H_, N_, PV3, vp_hi.shape[1], 0, 0, 1, N_,
                 _ptr(Tog), N_, F_ * H_ * N_, 1, 0, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
-        _check(lib().dfold_ipa_ds_bwd(*args, _ptr(dcat), _ptr(d_og), _ptr(delta), _ptr(dP), _ptr(Tz), _ptr(Tog), _ptr(dS), _ptr(dgamma),
+        _check(lib().dfold_ipa_ds_bwd(*args, _ptr(dcat), _ptr(d_og), _ptr(delta), _ptr(dP), _ptr(Tz), _ptr(Tog), _ptr(dS), _ptr(dgamma_part),
                                       None if pts_gemm else _ptr(dq_pts), _ptr(dkv_pts), _stream()), "dfold_ipa_ds_bwd")
+        dgamma = dgamma_part.sum(1)
         del Tz
         del dP
         del Tog
@@ -980,7 +992,7 @@ class _IpaAttnTCFn(Function):
             _check(lib().dfold_gemm_wgrad_bf16x3_batched(
                 _ptr(ds_hi), _ptr(ds_lo), N_, N_, F_ * H_, ds_hi.shape[1], N_ * ds_hi.shape[1],
                 _ptr(qn_hi), _ptr(qn_lo), 32, N_, F_ * H_, qn_hi.shape[1], N_ * qn_hi.shape[1],
-                32, 1, N_, F_ * H_, 1, 0, 1, 0, 1, 0,
+                32, 1, N_, F_ * H_, 0, 1, 0, 1, 0,
                 _ptr(g2), 32, N_ * 32, 1.0, _stream()), "dfold_gemm_wgrad_bf16x3_batched")
             g1 = g1.reshape(F_, H_, N_, 32)
             gam = gamma.reshape(1, H_, 1, 1)
@@ -988,20 +1000,19 @@ class _IpaAttnTCFn(Function):
             dq_pts.copy_(dq.permute(0, 2, 1, 3).reshape(q_pts.shape))
             dk = gam * (g2[..., :PQ3].reshape(F_, H_, N_, PQ3) - g2[..., PQ3:PQ3 + 1].reshape(F_, H_, N_, 1) * kq.permute(0, 2, 1, 3))
             dkv_pts.reshape(F_, N_, H_, W)[..., :PQ3] = dk.permute(0, 2, 1, 3)
-        # ---- dV[j,h,c] = sum_{f,i} P[f,h,i,j] dO[f,i,h,c]   (MN-major, split-K over frames, atomic accumulate) ----
+        # ---- dV[j,h,c] = sum_{f,i} P[f,h,i,j] dO[f,i,h,c]   (MN-major, K over all frames) ----
         dkv = torch.zeros_like(kv)
-        splits = max(1, min(F_, 16))
         _check(lib().dfold_gemm_wgrad_bf16x3_batched(
             _ptr(p_hi), _ptr(p_lo), N_, N_, F_ * H_, n8, N_ * n8,
             _ptr(dc_hi), _ptr(dc_lo), D, N_, F_, dc_hi.shape[1], N_ * dc_hi.shape[1],
-            C_, F_, N_, H_, splits, H_, 1, 1, 0, C_,
+            C_, F_, N_, H_, H_, 1, 1, 0, C_,
             _ptr(dkv, C_), H_ * 2 * C_, 2 * C_, 1.0, _stream()), "dfold_gemm_wgrad_bf16x3_batched")
         # ---- dV_pts[f,j,h,e] = sum_i P[f,h,i,j] d_og[f,i,h,e] ----
         tmp = new(F_ * H_, N_, PV3)
         _check(lib().dfold_gemm_wgrad_bf16x3_batched(
             _ptr(p_hi), _ptr(p_lo), N_, N_, F_ * H_, n8, N_ * n8,
             _ptr(dg_hi), _ptr(dg_lo), PV3, N_, F_ * H_, dg_hi.shape[1], N_ * dg_hi.shape[1],
-            PV3, 1, N_, F_ * H_, 1, 0, 1, 0, 1, 0,
+            PV3, 1, N_, F_ * H_, 0, 1, 0, 1, 0,
             _ptr(tmp), PV3, N_ * PV3, 1.0, _stream()), "dfold_gemm_wgrad_bf16x3_batched")
         dkv_pts.reshape(F_, N_, H_, W)[..., PQ3:] = tmp.reshape(F_, H_, N_, PV3).permute(0, 2, 1, 3)
         # ---- dZ[i,j,c] = sum_{f,h} P[f,h,i,j] dOpair[f,i,h,c] ----
@@ -1009,7 +1020,7 @@ class _IpaAttnTCFn(Function):
         _check(lib().dfold_gemm_wgrad_bf16x3_batched(
             _ptr(p_hi), _ptr(p_lo), N_, F_ * H_, N_, N_ * n8, n8,
             _ptr(do_hi), _ptr(do_lo), Cp, F_ * H_, N_, do_hi.shape[1], F_ * H_ * do_hi.shape[1],
-            Cp, 1, F_ * H_, N_, 1, 0, 1, 0, 1, 0,
+            Cp, 1, F_ * H_, N_, 0, 1, 0, 1, 0,
             _ptr(dpair), Cp, N_ * Cp, 1.0, _stream()), "dfold_gemm_wgrad_bf16x3_batched")
         dlogit0 = dS.sum(0, keepdim=True) if logit0.shape[0] == 1 else dS
         return dlogit0, dkv, dq_pts, dkv_pts, dpair, dquat, dtrans, None, dgamma, None, None, None, None, None

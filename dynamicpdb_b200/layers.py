@@ -1,7 +1,7 @@
 """Shared building blocks of the host-side mirror: the AlphaFold-style ``Linear`` with named initialisers
 (reference src/model/ipa_pytorch_dynamic.py:107-172 and openfold/model/primitives.py:102-167), ``LayerNorm``
 (primitives.py:170-199) and the invariant-point-attention driver used by both IPA variants.
-All arithmetic goes through ``kernels`` (hand-written sm_100a CUDA behind the C-ABI); no CPU fallback.
+All arithmetic goes through ``kernels`` (hand-written sm_90a CUDA behind the C-ABI); no CPU fallback.
 """
 import math
 from typing import Callable, List, Optional
@@ -82,7 +82,7 @@ def normal_init_(weights):
 
 class Linear(nn.Linear):
     """``nn.Linear`` with the AlphaFold named initialisers (ref :107-172); forward runs the split-precision
-    tcgen05 GEMM (or the SIMT kernel for tiny shapes) through ``kernels.linear``."""
+    wgmma GEMM (or the SIMT kernel for tiny shapes) through ``kernels.linear``."""
 
     def __init__(self, in_dim: int, out_dim: int, bias: bool = True, init: str = "default",
                  init_fn: Optional[Callable[[torch.Tensor, torch.Tensor], None]] = None):

@@ -7,7 +7,7 @@ as the reference path  se3_diffuser.calc_rot_score -> utils.quat_to_rotvec (src/
 so3_diffuser.torch_score (:274-305, use_cached_score=False) -> igso3_expansion (:9-49) / score (:71-117), and
 r3_diffuser.score (:169-177) — but the sigma(t) lookup stays on the device (the reference does
 ``du.move_to_np(t)``, a host synchronisation inside the model forward).  The reference's own ``SE3Diffuser`` can be
-passed instead; this class exists so bench / tests run where /root/reference is absent.
+passed instead; this class exists so bench / tests run without a checkout of the reference.
 """
 import numpy as np
 import torch

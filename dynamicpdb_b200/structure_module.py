@@ -1,7 +1,7 @@
 """Host-side mirror of ``openfold/model/structure_module.py`` (SURVEY.md §8 rows a4, a12, a16): ``AngleResnet``
 (the only class DFOLDv2 executes, ipa_pytorch_dynamic.py:10,754), the vanilla ``InvariantPointAttention``,
 ``BackboneUpdate``, the transition blocks and ``StructureModule`` with the reference's constructor arguments,
-forward signatures and parameter names.  Arithmetic runs on the sm_100a kernels through ``kernels``.
+forward signatures and parameter names.  Arithmetic runs on the sm_90a kernels through ``kernels``.
 """
 from typing import Optional, Sequence, Tuple
 

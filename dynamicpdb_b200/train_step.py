@@ -2,8 +2,8 @@
 
 The reference trainer wraps the model in ``DistributedDataParallel(find_unused_parameters=True)`` and calls
 ``loss.backward(); optimizer.step()`` from Python (train_DFOLD_dynamics.py:612-616, 660-668); that keeps working on top
-of this package (tests/test_cpu_ddp.py).  At B200 kernel speeds the ~2000 kernel launches of a step cost as much host
-time as device time, so the B200-native step is:
+of this package (tests/test_cpu_ddp.py).  At these kernel speeds the ~700 kernel launches of a step would cost host time
+comparable to the device time, so the step is:
 
     static input buffers  ->  [ forward + loss + backward + ONE flat NCCL all-reduce of the gradients + Adam ]  (one graph)
 
@@ -133,8 +133,8 @@ class TrainStep:
             _kernels.GRAD_ACCUMULATE_INPLACE = prev
         if self.world > 1 and self.opt is None and self.chunks > 1:
             # optional (DFOLD_ALLREDUCE_CHUNKS > 1): the gradient exchange in pieces, the Adam update of piece c running while
-            # piece c + 1 is on the wire.  Measured at 2 x B200 with 8 pieces: 118.3 ms per step vs 117.4 ms for the single
-            # 738 MB all-reduce (smaller NCCL operations lose more than the hidden 1 ms Adam gains) -> off by default.
+            # piece c + 1 is on the wire.  Smaller NCCL operations can lose more than the hidden Adam update gains, and
+            # the single 738 MB all-reduce is the default.
             n = self.flat_grad.numel()
             per = (n // self.chunks + 3) // 4 * 4
             bounds = [(a, min(n, a + per)) for a in range(0, n, per)]

@@ -1,4 +1,4 @@
-/* dfold_b200 — C ABI of the B200-native (sm_100a) DFOLDv2 score-network hot path.
+/* dfold_b200 — C ABI of the sm_90a (H100) DFOLDv2 score-network hot path.
  *
  * The reference (fudan-generative-vision/dynamicPDB) is pure Python/PyTorch and has no FFI of its own; the
  * boundary a maintainer binds is this shared library (libdfold_b200.so), loaded with ctypes by
@@ -24,13 +24,13 @@ int dfold_abi_version(void);
 /* Host-side helper: *id_out = id of the CUDA-graph capture `stream` is recording into, 0 when not capturing
  * (HOST pointer). */
 int dfold_capture_id(void* stream, unsigned long long* id_out);
-/* Development aid: non-NULL `buf` (DEVICE, 4 x int64 per CTA) makes every following tcgen05 GEMM launch record per CTA
- * {mainloop cycles, MMA-thread wait on operand stages, MMA-thread wait on accumulator drain, accumulate-warp wait};
+/* Development aid: non-NULL `buf` (DEVICE, 4 x int64 per CTA) makes every following tensor-core GEMM launch record per CTA
+ * {mainloop cycles, consumer wait on operand stages, producer wait on a free stage, 0};
  * NULL switches it off. */
 int dfold_debug_gemm_stats(long long* buf);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Split-precision tensor-core GEMM (tcgen05, bf16 x 3, fp32 accumulate in TMEM) and its operand preparation.
+ * Split-precision tensor-core GEMM (wgmma, bf16 x 3, fp32 accumulate in registers) and its operand preparation.
  * Replaces every nn.Linear on the path (src/model/ipa_pytorch_dynamic.py:284-305,590,757-796;
  * src/model/Dfold_network_dynamic.py:444-445; openfold/model/structure_module.py:58-59,102-110) and the
  * ConvNet's eight Conv2d(5x5) (src/model/ipa_pytorch_dynamic.py:664-706).
@@ -40,7 +40,8 @@ int dfold_debug_gemm_stats(long long* buf);
  *   hi/lo     : [R][ldo], columns [C, cpad) zero-filled           (nullable pair)
  *   hi_t/lo_t : [C][ldt] (transposed), columns [R, rpad) zeroed   (nullable pair)
  * pre_relu applies max(x,0) first; gate (nullable, row stride ldg) zeroes x where gate <= 0 (ReLU backward);
- * colsum (nullable, [C], pre-zeroed) receives the column sums of the gated input (bias gradient). */
+ * colsum (nullable, [C], pre-zeroed) receives the column sums of the gated input (bias gradient), added in a fixed
+ * order so that they are the same from run to run. */
 int dfold_split2d(const float* x, long R, long C, long ld, int pre_relu, const float* gate, long ldg,
                   uint16_t* hi, uint16_t* lo, long ldo, long cpad,
                   uint16_t* hi_t, uint16_t* lo_t, long ldt, long rpad, float* colsum, void* stream);
@@ -88,13 +89,13 @@ int dfold_gemm_bf16x3_batched(const uint16_t* a_hi, const uint16_t* a_lo, long a
                               float* out, long ldo, long out_rows, int o_f_div, long o_col_bstride, float alpha,
                               void* stream);
 
-/* Batched / split-K MN-major GEMM (the reduction runs over ROWS of both operands).  For z = zq * splits + zs:
- *   out[zq][m][n] (+)= alpha * sum_{f in split zs} sum_j A[f*a_f_mul + zq*a_z_mul][j][m] * B[f*b_f_mul + zq*b_z_mul][j][zq*b_n_zmul + n]
- * A planes: dims (M, a_mid, a_outer) with element strides (lda, a_ostride); B likewise.  splits > 1 accumulates with
- * atomicAdd into a pre-zeroed output.  Used for dV = P^T dO, dV_pts, dZ in the IPA backward. */
+/* Batched MN-major GEMM (the reduction runs over ROWS of both operands).  For z in [0, zcount):
+ *   out[z][m][n] = alpha * sum_{f < Fk} sum_j A[f*a_f_mul + z*a_z_mul][j][m] * B[f*b_f_mul + z*b_z_mul][j][z*b_n_zmul + n]
+ * A planes: dims (M, a_mid, a_outer) with element strides (lda, a_ostride); B likewise.  Used for dV = P^T dO, dV_pts, dZ
+ * in the IPA backward. */
 int dfold_gemm_wgrad_bf16x3_batched(const uint16_t* a_hi, const uint16_t* a_lo, long M, long a_mid, long a_outer, long lda,
                                     long a_ostride, const uint16_t* b_hi, const uint16_t* b_lo, long b_cols, long b_mid,
-                                    long b_outer, long ldb, long b_ostride, long Nn, long Fk, long Nr, int zcount, int splits,
+                                    long b_outer, long ldb, long b_ostride, long Nn, long Fk, long Nr, int zcount,
                                     int a_f_mul, int a_z_mul, int b_f_mul, int b_z_mul, long b_n_zmul,
                                     float* out, long ldo, long out_z_stride, float alpha, void* stream);
 
@@ -102,7 +103,7 @@ int dfold_gemm_wgrad_bf16x3_batched(const uint16_t* a_hi, const uint16_t* a_lo, 
  * the once-per-sample q.k logits and the reductions of the IPA backward.
  * C[b,b2][m][n] = act(alpha * sum_k A[m][k] * B[n][k] + bias[n]) + beta * R[m][n]; strides in elements
  * (*_rs row, *_cs column, *_bs outer batch, *_bs2 inner batch).  ksplit > 1: split-K with atomic accumulation into
- * a pre-zeroed C (no bias / residual / activation). */
+ * a pre-zeroed C (no bias / residual / activation; the last bits then vary from run to run). */
 int dfold_sgemm(const float* A, long a_rs, long a_cs, long a_bs, long a_bs2,
                 const float* B, long b_rs, long b_cs, long b_bs, long b_bs2,
                 float* C, long c_rs, long c_cs, long c_bs, long c_bs2,
@@ -120,7 +121,7 @@ int dfold_global_layernorm_fwd(const float* x, float* y, float* stats, double* w
 int dfold_global_layernorm_bwd(const float* x, const float* dy, const float* stats, double* workspace, float* dx,
                                long n, int silu, void* stream);
 /* nn.LayerNorm / openfold LayerNorm over the last axis (openfold/model/primitives.py:170-199). stats [rows][2].
- * dw, db must be pre-zeroed. */
+ * dw, db must be pre-zeroed; they are accumulated in a fixed order, so they are the same from run to run. */
 int dfold_row_layernorm_fwd(const float* x, const float* w, const float* b, float* y, float* stats, long rows, int C,
                             float eps, void* stream);
 int dfold_row_layernorm_bwd(const float* x, const float* w, const float* dy, const float* stats, float* dx, float* dw,
@@ -163,7 +164,8 @@ int dfold_ipa_attn_fwd(const float* logit0, long logit0_fstride, const float* kv
                        int dfold, float inf, float eps, float* out_cat, float* lse, void* stream);
 /* Backward: writes d_og [F,N,H,Pv,3], delta [F,H,N], P and dS [H,F,N,N] (workspaces the caller reduces into dv / dz /
  * d-logits with dfold_sgemm), dq_pts [F,N,H,Pq,3], the key-point part of dkv_pts [F,N,H,Pq+Pv,3], dquat / dtrans of
- * the local-frame transform, and accumulates dgamma [H] (pre-zeroed). */
+ * the local-frame transform, and per-CTA partials of dgamma: dgamma [H][F*N], zeroed by the caller, whose row h sums to
+ * d(gamma_h) (added by the caller in order: no atomics). */
 int dfold_ipa_attn_bwd(const float* logit0, long logit0_fstride, const float* kv, long kv_fstride, const float* q_pts,
                        const float* kv_pts, const float* pair, long pair_fstride, const float* quat, const float* trans,
                        const float* mask, const float* gamma, int F, int N, int H, int C, int Pq, int Pv, int Cp,
@@ -187,22 +189,21 @@ int dfold_ipa_pair_fwd(const float* logit0, long logit0_fstride, const float* q_
                        int dfold, float inf, float eps, float* out_cat, void* stream);
 /* Fused forward core (csrc/ipa_fused.cu), frame-shared logit0 [H,N,N] and pair [N,N,Cp]: one kernel does the point
  * distances (exact fp32), the exact two-pass softmax, the pair and value-point aggregations, the local-frame transform and
- * the concat layout; p_hi / p_lo (nullable: inference) receive the bf16 hi/lo probability planes for the backward GEMMs.
- * kv_hi / kv_lo: bf16 hi/lo planes of kv [N, H*2C] (row stride ldkv); when given (C = 256) the scalar values o = P V are
- * produced in the same kernel by tcgen05.mma from a shared-memory P tile into TMEM (P does not travel through HBM);
- * when null, columns [0, H*C) of the concat buffer are left to dfold_gemm_bf16x3_batched.  H=8, Pq=8, Pv=12, Cp=32.
+ * the concat layout; p_hi / p_lo receive the bf16 hi/lo probability planes, which feed the P V GEMM and the backward GEMMs:
+ * columns [0, H*C) of the concat buffer are left to dfold_gemm_bf16x3_batched.  H=8, Pq=8, Pv=12, Cp=32.
  * Replaces src/model/ipa_pytorch_dynamic.py:402-504. */
 int dfold_ipa_fused_fwd(const float* logit0, const float* q_pts, const float* kv_pts, const float* pair, const float* quat,
                         const float* trans, const float* mask, const float* gamma, uint16_t* p_hi, uint16_t* p_lo, long ldp,
-                        const uint16_t* kv_hi, const uint16_t* kv_lo, long ldkv, int F, int N, int H, int C, int Pq, int Pv,
-                        int Cp, int dfold, float inf, float eps, float* out_cat, void* stream);
+                        int F, int N, int H, int C, int Pq, int Pv, int Cp, int dfold, float inf, float eps, float* out_cat,
+                        void* stream);
 /* Development aid: per-CTA cycle counters of the next dfold_ipa_fused_fwd launches (16 x int64 per CTA; null = off). */
 int dfold_debug_ipa_stats(long long* buf);
 /* Epilogue backward: d_og [F,N,H,Pv,3], delta [F,H,N], dquat [F,N,4], dtrans [F,N,3]. */
 int dfold_ipa_pre_bwd(const float* quat, const float* trans, int F, int N, int H, int C, int Pv, int Cp, int dfold,
                       const float* out_cat, const float* dcat, float* d_og, float* delta, float* dquat, float* dtrans,
                       void* stream);
-/* dS = P (dP + d_og.v_pts + dO_pair.z - delta) [F,H,N,N], dgamma [H] (pre-zeroed), dq_pts, key part of dkv_pts.
+/* dS = P (dP + d_og.v_pts + dO_pair.z - delta) [F,H,N,N], dgamma partials [H][F*N] as dfold_ipa_attn_bwd, dq_pts, key
+ * part of dkv_pts.
  * Tz (nullable) = the dO_pair.z term precomputed as [N(i)][F*H][N(j)] by dfold_gemm_bf16x3_batched.
  * Tog (nullable; needs Tz and Pq = 8) = the value-point term d_og.v_pts precomputed as [F,H,N,N] the same way: the kernel then
  * keeps each key's points in registers and only adds, scales and accumulates d(gamma).  dq_pts null: the caller computes

@@ -1,6 +1,6 @@
 """Dump the numeric residue tables the score-network epilogue reads (SURVEY.md §2 row 17:
 "constants are *read* by the hot path; import as-is") into dynamicpdb_b200/data/residue_tables.npz,
-so the product and the oracle run on the GPU box where /root/reference does not exist.
+so the product and the oracle run without a checkout of the reference.
 
 Sources (reference file:line):
   src/data/residue_constants.py:778-781  restype_atom14_to_rigid_group / _mask / _rigid_group_positions,

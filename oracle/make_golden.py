@@ -1,4 +1,4 @@
-"""Generate tests/golden/*.pt from the UNMODIFIED reference (run here, where /root/reference is mounted):
+"""Generate tests/golden/*.pt from the UNMODIFIED reference (a checkout of it at $DFOLD_REFERENCE_ROOT):
 
     python oracle/make_golden.py
 
@@ -65,10 +65,13 @@ def run_net(name, c):
     print(name, "loss", float(loss), "params", len(sd))
 
 
+FRAMES_A256 = [0, 31, 62, 63]
+
+
 def run_net_big(name="net_A256", nf=64, N=256, seed=7):
     """The BENCHED shape (BASELINE.json configs[2]: preset A, 64 frames x 256 residues), forward only under no_grad
-    (the unmodified reference materialises [nf,N,N,H,Pq,3] tensors; ~25 GB peak).  Stores every small output whole and
-    the last two frames of the atom tensors."""
+    (the unmodified reference materialises [nf,N,N,H,Pq,3] tensors; ~25 GB peak).  Stores the frames FRAMES_A256 of every
+    output but the atom tensors, the last two frames of those, and the surrogate loss over all frames (under 1 MB)."""
     c = dict(preset="PRESET_A", nf=nf, N=N, seed=seed)
     conf = syn.model_conf(nf, **syn.PRESET_A)
     net = RefNet.FullScoreNetwork(conf, se3_diffuser.SE3Diffuser(syn.diffuser_conf(1.0)))
@@ -79,8 +82,8 @@ def run_net_big(name="net_A256", nf=64, N=256, seed=7):
     keep = {}
     for k, v in out.items():
         v = v.detach()
-        keep[k] = v[-2:].clone() if k in ("atom37", "atom14") else v.clone()
-    torch.save({"case": c, "shapes": {k: tuple(v.shape) for k, v in sd.items()}, "out": keep,
+        keep[k] = v[-2:].clone() if k in ("atom37", "atom14") else v[FRAMES_A256].clone()
+    torch.save({"case": c, "shapes": {k: tuple(v.shape) for k, v in sd.items()}, "out": keep, "frames": FRAMES_A256,
                 "loss": float(syn.surrogate_loss(out))}, os.path.join(OUT, name + ".pt"))
     print(name, "loss", float(syn.surrogate_loss(out)))
 
@@ -249,7 +252,50 @@ def run_loader():
     print("[golden] loader:", {k: tuple(v.shape) for k, v in res.items()})
 
 
+def boundary_batch():
+    """The batch of the boundary fixture (shared with tests/test_cpu_boundary.py)."""
+    feats = syn.add_loss_targets(syn.make_feats(3, 12, seed=21, loader_dtypes=True), seed=21)
+    feats["fixed_mask"][:, 2] = 1
+    return feats
+
+
+def run_boundary():
+    """The reference's own caller: Experiment.loss_fn (train_DFOLD_dynamics.py:1181) driving the reference network on
+    boundary_batch() (loss, aux_data, every parameter gradient), and one plain forward of the reference network on
+    loader-dtype features (tiny preset, 3 frames x 14 residues).  Weights: synthetic.random_state, seeds 131 / 132."""
+    from types import SimpleNamespace
+    from oracle import dfold_oracle as O
+    ref_shims.install_trainer_stubs()
+    diffuser = se3_diffuser.SE3Diffuser(syn.diffuser_conf(1.0))
+    net = RefNet.FullScoreNetwork(syn.model_conf(3, **syn.PRESET_TINY), diffuser)
+    net.load_state_dict(syn.random_state({k: v.shape for k, v in net.state_dict().items()}, seed=131))
+    model_conf = SimpleNamespace(cfg_drop_in_train=True, cfg_drop_rate=0.0, embed=SimpleNamespace(embed_self_conditioning=False))
+    exp = ref_shims.reference_experiment(net, diffuser, model_conf, O.default_exp_conf(**BOUNDARY_EXP_CONF),
+                                         SimpleNamespace(diffuse_rot=True))
+    exp._conf = SimpleNamespace(model=SimpleNamespace(cfg_drop_rate=0.0, cfg_gamma=1.0))
+    exp._data_conf = SimpleNamespace(num_t=4, min_t=0.01)
+    loss, aux = exp.loss_fn(boundary_batch())
+    loss.backward()
+    grads = {k: p.grad.detach().clone() for k, p in net.named_parameters() if p.grad is not None}
+    grad_norms = {k: float(g.norm()) for k, g in grads.items()}
+    grads = {k: g for k, g in grads.items() if g.numel() <= 4096}           # small gradients whole, norms of all
+    net2 = RefNet.FullScoreNetwork(syn.model_conf(3, **syn.PRESET_TINY), diffuser)
+    net2.load_state_dict(syn.random_state({k: v.shape for k, v in net2.state_dict().items()}, seed=132))
+    with torch.no_grad():
+        fwd = net2(syn.make_feats(3, 14, seed=9, loader_dtypes=True))
+    torch.save({"loss": loss.detach(), "aux": {k: v.detach() if torch.is_tensor(v) else v for k, v in aux.items()},
+                "grads": grads, "grad_norms": grad_norms, "forward": {k: v.detach() for k, v in fwd.items()}}, os.path.join(OUT, "boundary.pt"))
+    print("[golden] boundary: loss", float(loss.detach()), "grads", len(grad_norms))
+
+
+BOUNDARY_EXP_CONF = dict(bb_atom_loss_weight=1.0, bb_atom_loss_t_filter=0.25, dist_mat_loss_weight=1.0,
+                         dist_mat_loss_t_filter=0.25, aux_loss_weight=0.25)
+
+
 if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "boundary":
+        run_boundary()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "loader":
         run_loader()
         sys.exit(0)
@@ -270,3 +316,4 @@ if __name__ == "__main__":
         run_net(n, c)
     run_vanilla()
     run_rigid()
+    run_boundary()

@@ -1,8 +1,8 @@
-"""Import shims that let the UNMODIFIED reference (/root/reference) be imported in this container.
+"""Import shims that let the UNMODIFIED reference (a checkout at $DFOLD_REFERENCE_ROOT) be imported here.
 
 TEST INFRASTRUCTURE ONLY.  Nothing in the product path (dynamicpdb_b200/) may import this file.
 It is used by oracle/make_golden.py (fixture generation) and by the CPU tests that pin the oracle
-restatement against the live reference when /root/reference is mounted.
+restatement against the live reference when that checkout is present.
 
 The reference imports five packages at module-import time that are not installed here
 (SURVEY.md §8c): tree (openfold/np/residue_constants.py:24), deepspeed
@@ -15,7 +15,7 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("DFOLD_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("DFOLD_REFERENCE_ROOT", "")
 
 
 def reference_available() -> bool:

@@ -1,4 +1,4 @@
-"""Drop-in for the reference's src/model/ipa_pytorch_dynamic.py: re-exports the B200-native implementation."""
+"""Drop-in for the reference's src/model/ipa_pytorch_dynamic.py: re-exports the H100-native implementation."""
 from dynamicpdb_b200.ipa_pytorch_dynamic import *  # noqa: F401,F403
 from dynamicpdb_b200.ipa_pytorch_dynamic import (  # noqa: F401
     Linear, StructureModuleTransition, EdgeTransition, InvariantPointAttention, TorsionAngles, ScoreLayer,

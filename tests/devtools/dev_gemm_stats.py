@@ -1,4 +1,4 @@
-"""Development probe: where does the tcgen05 GEMM's MMA-issuing thread wait?  (python tests/devtools/dev_gemm_stats.py)"""
+"""Development probe: where do the tensor-core GEMM's producer and consumers wait?  (python tests/devtools/dev_gemm_stats.py)"""
 import math, sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import torch

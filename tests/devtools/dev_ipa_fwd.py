@@ -27,9 +27,9 @@ def run(train):
 
 
 outs = {}
-for name, unf, tc, train in (("fused+tcgen05 train", "0", "1", True), ("fused+tcgen05 infer", "0", "1", False),
-                             ("fused + P.V GEMM  ", "0", "0", True), ("three kernels     ", "1", "0", True)):
-    os.environ["DFOLD_IPA_UNFUSED"], os.environ["DFOLD_IPA_FUSED_TC"] = unf, tc
+for name, unf, train in (("fused train       ", "0", True), ("fused infer       ", "0", False),
+                         ("three kernels     ", "1", True)):
+    os.environ["DFOLD_IPA_UNFUSED"] = unf
     for _ in range(3):
         outs[name] = run(train)
     torch.cuda.synchronize()

@@ -1,5 +1,5 @@
 """Development probe: time of the fused IPA forward with individual phases disabled (DFOLD_IPA_DEBUG_SKIP bit mask:
-1 pass 1, 2 distances of pass 2, 4 pair aggregation, 8 value points, 16 tcgen05 MMAs).  Results are wrong by design."""
+1 pass 1, 2 distances of pass 2, 4 pair aggregation, 8 value points).  Results are wrong by design."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import torch

@@ -1,4 +1,4 @@
-"""Development probe: per-shape time of the tcgen05 GEMM launches of one eager training step."""
+"""Development probe: per-shape time of the tensor-core GEMM launches of one eager training step."""
 import sys, os, collections
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import torch

@@ -116,7 +116,7 @@ def test_c_abi_exports_every_declared_symbol():
     for name in declared:
         assert isinstance(getattr(L, name), ctypes._CFuncPtr), name
     assert declared == set(kernels.exported_symbols())
-    assert L.dfold_abi_version() == 2
+    assert L.dfold_abi_version() == 3
 
 
 def test_ctypes_signatures_match_the_header():
@@ -151,17 +151,38 @@ def test_ops_refuse_cpu_tensors():
         featurize_window(torch.zeros(2, 5, 37, 3), torch.ones(5, 37), torch.zeros(5, dtype=torch.long))
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/src"), reason="reference checkout not mounted")
-def test_import_overlay_shadows_only_the_hot_path():
+def _skeleton_reference(root):
+    """A stand-in for the original project's package layout (namespace packages src / src.model / src.data /
+    openfold.utils, regular packages openfold / openfold.model / openfold.np): one marker module per file."""
+    files = ["src/model/ipa_pytorch_dynamic.py", "src/model/Dfold_network_dynamic.py", "src/model/utils.py",
+             "src/data/se3_diffuser.py", "openfold/__init__.py", "openfold/model/__init__.py",
+             "openfold/model/structure_module.py", "openfold/np/__init__.py", "openfold/np/residue_constants.py",
+             "openfold/utils/rigid_utils.py", "openfold/utils/tensor_utils.py"]
+    for f in files:
+        path = os.path.join(root, f)
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        with open(path, "w") as fh:
+            fh.write("SKELETON = True\n")
+
+
+def test_import_overlay_shadows_only_the_hot_path(tmp_path):
+    """overlay/ first on sys.path: the four hot-path modules resolve to the overlay, everything else of the reference
+    (here a skeleton of its layout) still resolves to the reference tree."""
+    ref = str(tmp_path / "reference")
+    _skeleton_reference(ref)
     code = ("import sys; sys.path[:0]=[%r, %r]; from oracle import ref_shims; ref_shims.install();"
-            "import src.model.ipa_pytorch_dynamic as a, openfold.utils.rigid_utils as c, openfold.model.structure_module as d,"
-            "src.data.se3_diffuser as e, openfold.np.residue_constants as f; "
-            "print(a.__file__, c.__file__, d.__file__, e.__file__, f.__file__)") % (os.path.join(ROOT, "overlay"), ROOT)
-    out = subprocess.run([sys.executable, "-W", "ignore", "-c", code], capture_output=True, text=True, timeout=300)
+            "import src.model.ipa_pytorch_dynamic as a, src.model.Dfold_network_dynamic as b, openfold.utils.rigid_utils as c,"
+            "openfold.model.structure_module as d, src.data.se3_diffuser as e, openfold.np.residue_constants as f,"
+            "openfold.utils.tensor_utils as g, src.model.utils as h; "
+            "print(a.__file__, b.__file__, c.__file__, d.__file__, e.__file__, f.__file__, g.__file__, h.__file__)"
+            ) % (os.path.join(ROOT, "overlay"), ROOT)
+    env = dict(os.environ, DFOLD_REFERENCE_ROOT=ref)
+    out = subprocess.run([sys.executable, "-W", "ignore", "-c", code], capture_output=True, text=True, timeout=300, env=env)
     assert out.returncode == 0, out.stderr[-2000:]
-    a, c, d, e, f = out.stdout.split()[-5:]
-    assert all(p.startswith(os.path.join(ROOT, "overlay")) for p in (a, c, d))
-    assert e.startswith("/root/reference") and f.startswith("/root/reference")
+    paths = out.stdout.split()[-8:]
+    overlay = os.path.join(ROOT, "overlay") + os.sep
+    assert all(p.startswith(overlay) for p in paths[:4]), paths
+    assert all(p.startswith(ref + os.sep) for p in paths[4:]), paths
 
 
 def test_dead_frame_elimination_is_exact(oracle_ops, monkeypatch):

@@ -45,9 +45,8 @@ def _net(nf, preset):
 
 def test_device_sampler_matches_literal_loop(monkeypatch):
     """One trunk pass + per-step score / reverse kernels == evaluating the whole network at every step (same noise).
-    The split-K GEMM accumulates with atomics (run-to-run rounding noise, which u / |u| of a near-zero torsion amplifies
-    without bound); the comparison of two runs needs the deterministic schedule."""
-    monkeypatch.setenv("DFOLD_GEMM_NO_SPLITK", "1")
+    The comparison of two runs relies on the kernels' fixed accumulation order (run-to-run rounding noise would be amplified
+    without bound by u / |u| of a near-zero torsion)."""
     nf, N, num_t = 3, 24, 7
     net = _net(nf, syn.PRESET_TINY)
     feats = {k: v.to(DEV) for k, v in syn.make_feats(nf, N, seed=6).items()}
@@ -65,8 +64,7 @@ def test_device_sampler_matches_literal_loop(monkeypatch):
 
 def test_graphed_sampler_replays_match_eager(monkeypatch):
     """The trunk pass + every score / reverse step captured in one CUDA graph: replays with new inputs reproduce the eager
-    loop (injected noise, deterministic GEMM schedule)."""
-    monkeypatch.setenv("DFOLD_GEMM_NO_SPLITK", "1")
+    loop (injected noise, fixed accumulation order)."""
     nf, N, num_t = 3, 24, 6
     net = _net(nf, syn.PRESET_TINY)
     g = torch.Generator().manual_seed(2)
@@ -86,7 +84,6 @@ def test_graphed_sampler_replays_match_eager(monkeypatch):
 
 def test_memoized_network_on_gpu_and_cache_invalidation(monkeypatch):
     """MemoizedScoreNetwork on CUDA: a new window allocated at the same address must NOT hit the cache (ADVICE r1)."""
-    monkeypatch.setenv("DFOLD_GEMM_NO_SPLITK", "1")       # two evaluations are compared at 1e-6: deterministic schedule
     nf, N = 3, 16
     net = _net(nf, syn.PRESET_TINY)
     memo = MemoizedScoreNetwork(net)

@@ -21,11 +21,12 @@ def _per_residue_l2(a, b):
 
 
 def _record(case, errs):
-    """Measured parity errors -> gpurun_out/parity_errors.json (quoted in DESIGN.md)."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    path = os.path.join(root, "gpurun_out", "parity_errors.json")
+    """Measured parity errors -> the JSON file named by $DFOLD_PARITY_ERRORS, when set (DESIGN.md §2)."""
+    path = os.environ.get("DFOLD_PARITY_ERRORS")
+    if not path:
+        return
     try:
-        os.makedirs(os.path.dirname(path), exist_ok=True)
+        os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
         d = json.load(open(path)) if os.path.exists(path) else {}
         d[case] = errs
         json.dump(d, open(path, "w"), indent=1, sort_keys=True)

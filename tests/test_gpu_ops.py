@@ -94,7 +94,7 @@ def unit(*s, grad=True):
 
 
 def test_library_loads():
-    assert K.lib().dfold_abi_version() == 2
+    assert K.lib().dfold_abi_version() == 3
 
 
 @pytest.mark.parametrize("M,Kd,N", [(5, 3, 16), (70, 14, 32), (33, 7, 6), (256, 160, 6), (100, 128, 8), (4096, 7, 6), (3000, 14, 32)])

@@ -23,7 +23,6 @@ def _net(nf, preset):
 
 
 def test_graph_replay_matches_eager_steps(monkeypatch):
-    monkeypatch.setenv("DFOLD_GEMM_NO_SPLITK", "1")      # two runs are compared: keep the GEMM accumulation order fixed
     nf, N = 3, 24
     feats = {k: v.cuda() for k, v in syn.make_feats(nf, N, seed=4).items()}
     base = _net(nf, syn.PRESET_TINY)
@@ -42,12 +41,32 @@ def test_graph_replay_matches_eager_steps(monkeypatch):
     # gradients of every step agree (parameters themselves are not compared element-wise: Adam turns the noise-level
     # gradients of mathematically gradient-free parameters, e.g. linear_b.bias, into +-lr moves of arbitrary sign)
     for ga, gb in zip(runs[True][2], runs[False][2]):
-        assert ((ga - gb).norm() / gb.norm()).item() < 5e-3      # the IPA backward still accumulates dV / d(gamma) atomically
+        assert ((ga - gb).norm() / gb.norm()).item() < 5e-3
     # parameters that receive no gradient (dead-output embedder, linear_rbf) are not moved by Adam
     for k, v in base.state_dict().items():
         if k.startswith("embedding_layer.") or "linear_rbf" in k:
             assert torch.equal(runs[True][1][k], v), k
     assert runs[True][0][-1] < runs[True][0][0]            # the loss goes down
+
+
+def test_training_steps_are_reproducible():
+    """Two runs of the same captured training steps from the same weights and inputs give bit-identical losses, gradients
+    and parameters.  Preset A at 8 frames has the small, long-K launches (the last layers of the dead-frame pyramid, the
+    IPA dV over frames) and the bias-gradient / d(gamma) reductions that an order-dependent (atomic) reduction would
+    make differ; Adam would amplify such differences of noise-level gradients to +-lr moves."""
+    nf, N = 8, 64
+    feats = {k: v.cuda() for k, v in syn.make_feats(nf, N, seed=3).items()}
+    runs = []
+    for _ in range(2):
+        net = _net(nf, syn.PRESET_A)
+        ts = TrainStep(net, syn.surrogate_loss, feats, lr=1e-4, graph=True, warmup=2)
+        losses = [ts().clone() for _ in range(3)]
+        torch.cuda.synchronize()
+        runs.append((torch.stack(losses).cpu(), ts.flat_grad.cpu(), ts.flat_param.cpu()))
+        del net, ts
+        torch.cuda.empty_cache()
+    for a, b, what in zip(runs[0], runs[1], ("loss", "gradients", "parameters")):
+        assert torch.equal(a, b), f"{what} differ between two identical runs: max |diff| {(a - b).abs().max().item():.3e}"
 
 
 def test_long_chain_1024_residues_forward_backward():
@@ -91,7 +110,6 @@ def test_fused_adam_matches_torch_adam_amsgrad():
 def test_train_step_gradients_equal_plain_autograd(monkeypatch):
     """The step accumulates the shared ConvNet's weight gradients in place (kernels.GRAD_ACCUMULATE_INPLACE) and updates flat
     parameter views: its gradient buffer must equal what loss.backward() gives on an untouched copy of the network."""
-    monkeypatch.setenv("DFOLD_GEMM_NO_SPLITK", "1")
     nf, N = 3, 24
     feats = {k: v.cuda() for k, v in syn.make_feats(nf, N, seed=4).items()}
     base = _net(nf, syn.PRESET_TINY)
