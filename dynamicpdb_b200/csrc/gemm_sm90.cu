@@ -625,12 +625,20 @@ extern "C" int dfold_gemm_bf16x3_batched(
     DFOLD_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "dfold_gemm_bf16x3_batched: lda/ldb must be multiples of 8");
     DFOLD_REQUIRE(a_k_bstride % 8 == 0 && b_k_ofs % 8 == 0 && b_k_bstride % 8 == 0,
                   "dfold_gemm_bf16x3_batched: K offsets must be multiples of 8 elements (TMA 16-byte alignment)");
+    // K tail: the A / B boxes may run past [k_ofs, k_ofs + K) into the neighbouring batch slice; require K % 64 == 0
+    const bool k_sliced = a_k_bstride != 0 || b_k_ofs != 0 || b_k_bstride != 0;
+    DFOLD_REQUIRE(K % BK == 0 || !k_sliced,
+                  "dfold_gemm_bf16x3_batched: K must be a multiple of 64 when it is a slice of a wider row");
+    // Unsliced, the reduction covers columns [0, K): the maps end there, so a K tail reads the out-of-bounds zero fill
+    // and not the columns of rows that are wider than K.
+    const long a_k_end = k_sliced ? a_cols : (a_cols < K ? a_cols : K);
+    const long b_k_end = k_sliced ? b_cols : (b_cols < K ? b_cols : K);
     const int bn = pick_bn(n_out, n_batches * cdiv(Nr, BM));
     CUtensorMap maps[4];
-    if (make_map(&maps[0], a_hi, a_cols, Nr, a_frames, lda, Nr * lda, BK, BM, 1)) return 1;
-    if (make_map(&maps[1], a_lo, a_cols, Nr, a_frames, lda, Nr * lda, BK, BM, 1)) return 1;
-    if (make_map(&maps[2], b_hi, b_cols, b_rows, b_z, ldb, b_rows * ldb, BK, bn, 1)) return 1;
-    if (make_map(&maps[3], b_lo, b_cols, b_rows, b_z, ldb, b_rows * ldb, BK, bn, 1)) return 1;
+    if (make_map(&maps[0], a_hi, a_k_end, Nr, a_frames, lda, Nr * lda, BK, BM, 1)) return 1;
+    if (make_map(&maps[1], a_lo, a_k_end, Nr, a_frames, lda, Nr * lda, BK, BM, 1)) return 1;
+    if (make_map(&maps[2], b_hi, b_k_end, b_rows, b_z, ldb, b_rows * ldb, BK, bn, 1)) return 1;
+    if (make_map(&maps[3], b_lo, b_k_end, b_rows, b_z, ldb, b_rows * ldb, BK, bn, 1)) return 1;
     GemmParams p{};
     p.mode = 0;
     p.kc = (int)cdiv(K, BK);
@@ -647,9 +655,6 @@ extern "C" int dfold_gemm_bf16x3_batched(
     p.bmod = bmod; p.a_f_div = a_f_div; p.a_k_bstride = (int)a_k_bstride;
     p.b_k_ofs = (int)b_k_ofs; p.b_k_bstride = (int)b_k_bstride; p.b_z_bstride = b_z_bstride;
     p.o_f_div = o_f_div; p.o_col_bstride = o_col_bstride;
-    // K tail: the A / B boxes may run past [k_ofs, k_ofs + K) into the neighbouring batch slice; require K % 64 == 0
-    DFOLD_REQUIRE(K % BK == 0 || (a_k_bstride == 0 && b_k_ofs == 0 && b_k_bstride == 0),
-                  "dfold_gemm_bf16x3_batched: K must be a multiple of 64 when it is a slice of a wider row");
     dim3 grid((unsigned)cdiv(n_out, bn), (unsigned)(n_batches * p.tiles_per_frame), 1);
     cudaStream_t st = as_stream(stream);
     if (bn == 128) return launch<128>(maps, p, grid, st);

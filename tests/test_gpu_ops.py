@@ -1,6 +1,7 @@
 """-m gpu: every CUDA operator (through the C-ABI) against the plain-torch oracle, forward and backward.
 
-The oracle side runs in float64 on the CPU so the reported error is the CUDA kernel's own error.  Tolerances are
+The oracle side runs in float64 (on the CPU; on the GPU for the full-width convolutions and sequences longer than 512) so
+the reported error is the CUDA kernel's own error.  Tolerances are
 relative to the largest reference magnitude of each tensor:
   * fp32 CUDA-core kernels: 2e-5
   * split-bf16 (x3) tensor-core GEMM / convolution: 1e-4 (hi/lo split keeps ~16 mantissa bits per operand)
@@ -63,10 +64,28 @@ def _safe_gate(pre, tau=1e-3):
     return (pre.abs() > tau * pre.abs().max()).to(torch.float64)
 
 
-def check(name, inputs, tol, post=None, wmask=None, grad_tol=None, **kwargs):
+REF_PEAK_BYTES = 16 << 30      # the float64 oracle on the GPU stays under 16 GB (the device is shared)
+
+
+def _ref_device(work):
+    """Where the float64 oracle runs: the CPU, or the GPU for problems the CPU would take minutes over."""
+    return DEV if work > 5e10 else "cpu"
+
+
+def check(name, inputs, tol, post=None, wmask=None, grad_tol=None, ref_device="cpu", **kwargs):
     fo = getattr(O, name) if post is None else (lambda *a, **k: post(getattr(O, name)(*a, **k), *a))
     fk = getattr(K, name) if post is None else (lambda *a, **k: post(getattr(K, name)(*a, **k), *a))
-    ro, rg = _run(fo, inputs, kwargs, torch.float64, "cpu", wmask)
+    if ref_device == "cpu":
+        ro, rg = _run(fo, inputs, kwargs, torch.float64, "cpu", wmask)
+    else:
+        torch.cuda.synchronize()
+        base = torch.cuda.memory_allocated()
+        torch.cuda.reset_peak_memory_stats()
+        ro, rg = _run(fo, inputs, kwargs, torch.float64, ref_device, wmask)
+        peak = torch.cuda.max_memory_allocated() - base
+        print(f"{name}: float64 reference peak {peak / 2**30:.2f} GB")
+        assert peak < REF_PEAK_BYTES, f"{name}: the float64 reference took {peak / 2**30:.1f} GB of device memory"
+        torch.cuda.empty_cache()
     co, cg = _run(fk, inputs, kwargs, torch.float32, DEV, wmask)
     torch.cuda.synchronize()
     for i, (a, b) in enumerate(zip(ro, co)):
@@ -115,16 +134,32 @@ def test_linear_tensor_core(M, Kd, N, act, pre_relu, res):
     check("linear", inputs, 1e-4, wmask=wmask, act=act, pre_relu=pre_relu, residual=R(M, N) if res else None)
 
 
-@pytest.mark.parametrize("F,N,Ci,Co", [(2, 16, 160, 80), (3, 12, 80, 160), (5, 130, 64, 128), (8, 256, 320, 256), (1, 40, 256, 640)])
+def _conv_ref_device(F, N, Ci, Co):
+    return DEV if F * N * Ci * Co > 1e9 else "cpu"
+
+
+@pytest.mark.parametrize("F,N,Ci,Co", [(2, 16, 160, 80), (3, 12, 80, 160), (5, 130, 64, 128), (8, 256, 320, 256), (1, 40, 256, 640),
+                                       (8, 256, 1280, 640), (8, 256, 640, 1280)])      # the ConvNet's widths
 @pytest.mark.parametrize("relu,res", [(True, False), (True, True), (False, False)])
 def test_conv5x5(F, N, Ci, Co, relu, res):
     inputs = [R(F, N, Ci), R(Co, Ci, 5, 5, scale=1.0 / math.sqrt(25 * Ci)), R(Co)]
     residual = R(F, N, Co) if res else None
+    dev = _conv_ref_device(F, N, Ci, Co)
     wmask = None
     if relu:
         with torch.no_grad():
-            wmask = _safe_gate(O.conv5x5(*[t.double() for t in inputs], relu=False))
-    check("conv5x5", inputs, 1e-4, wmask=wmask, relu=relu, residual=residual)
+            wmask = _safe_gate(O.conv5x5(*[t.double().to(dev) for t in inputs], relu=False)).cpu()
+    check("conv5x5", inputs, 1e-4, wmask=wmask, relu=relu, residual=residual, ref_device=dev)
+
+
+def test_conv5x5_bench_shape():
+    """Forward and backward of the first ConvNet layer at the benchmark shape: 64 frames x 256 residues, 1280 -> 640
+    channels, a 32000-long reduction per output in the forward and 16384 pixels per weight-gradient tap."""
+    F, N, Ci, Co = 64, 256, 1280, 640
+    inputs = [R(F, N, Ci), R(Co, Ci, 5, 5, scale=1.0 / math.sqrt(25 * Ci)), R(Co)]
+    with torch.no_grad():
+        wmask = _safe_gate(O.conv5x5(*[t.double().to(DEV) for t in inputs], relu=False)).cpu()
+    check("conv5x5", inputs, 1e-4, wmask=wmask, relu=True, ref_device=DEV)
 
 
 @pytest.mark.parametrize("shape", [(3, 12, 32), (8, 256, 256), (1, 7, 5)])
@@ -187,30 +222,39 @@ def _ipa_inputs(F, N, H, C, Pq, Pv, Cp, Fs, Fz, masked):
     (2, 136, 4, 64, 4, 6, 16, 1, 1, False),    # tensor-core path, vanilla layout, N not a multiple of 64
     (2, 33, 4, 16, 4, 8, 64, 2, 2, False),     # vanilla OpenFold, batched z and per-frame s
     (3, 70, 2, 8, 2, 3, 4, 3, 1, True),        # per-frame s, shared z, N not a multiple of the tiles
+    (1, 1024, 8, 256, 8, 12, 32, 1, 1, True),  # preset A at the long-chain benchmark length
+    (2, 1000, 8, 256, 8, 12, 32, 1, 1, True),  # N not a multiple of 32, 64 or 128
+    (1, 1280, 8, 256, 8, 12, 32, 1, 1, True),  # the longest N of the tensor-core path
+    (1, 1288, 8, 256, 8, 12, 32, 1, 1, True),  # the first N past it: csrc/ipa_attn.cu (shared memory independent of N)
+    (2, 72, 4, 64, 12, 6, 16, 1, 1, True),     # tensor-core path with 3 Pq > 31: point gradients in ipa_pts_grad_kernel
+    (1, 616, 4, 64, 4, 8, 64, 1, 1, True),     # non-fused, N (H + Cp) > 40960 floats: ipa_pair_fwd reads z unstaged
 ])
 @pytest.mark.parametrize("masked", [False, True])
 def test_ipa_attention(F, N, H, C, Pq, Pv, Cp, Fs, Fz, dfold, masked):
     inputs = _ipa_inputs(F, N, H, C, Pq, Pv, Cp, Fs, Fz, masked)
+    dev = DEV if N > 512 else "cpu"
     # rows of masked QUERY residues see every logit shifted by -1e5: in fp32 (reference and kernel alike) that
     # quantises the logits to 2^-7, so those rows are compared only through the unmasked ones
     post = lambda out, *a: out * a[7][:, :, None]
     # d(gamma) [H] (gradient 7: the mask carries none) is a signed sum over all F*N*N pairs of a head whose terms are orders
     # of magnitude larger than the sum: the fp32 rounding of the logits alone moves it by ~2e-4 relative, run to run with the
     # atomic accumulation order, and the split-bf16 value-point term of dS (2^-17 per product) by up to ~7e-4
-    check("ipa_attention", inputs, 2e-4, post=post, grad_tol={7: 1.5e-3}, Pq=Pq, Pv=Pv, dfold=dfold, inf=1e5, eps=1e-8)
+    check("ipa_attention", inputs, 2e-4, post=post, grad_tol={7: 1.5e-3}, ref_device=dev, Pq=Pq, Pv=Pv, dfold=dfold, inf=1e5,
+          eps=1e-8)
 
 
-@pytest.mark.parametrize("F,N,Ci,Co,crop", [(7, 24, 64, 128, 2), (17, 40, 160, 80, 2), (5, 130, 128, 64, 4)])
+@pytest.mark.parametrize("F,N,Ci,Co,crop", [(7, 24, 64, 128, 2), (17, 40, 160, 80, 2), (5, 130, 128, 64, 4), (8, 256, 1280, 640, 3)])
 @pytest.mark.parametrize("relu,res", [(True, True), (False, False)])
 def test_conv5x5_cropped(F, N, Ci, Co, crop, relu, res):
     """Only the last F - crop output frames (dead-frame pyramid): forward, data gradient and weight gradient."""
     inputs = [R(F, N, Ci), R(Co, Ci, 5, 5, scale=1.0 / math.sqrt(25 * Ci)), R(Co)]
     residual = R(F - crop, N, Co) if res else None
+    dev = _conv_ref_device(F, N, Ci, Co)
     wmask = None
     if relu:
         with torch.no_grad():
-            wmask = _safe_gate(O.conv5x5(*[t.double() for t in inputs], relu=False, crop=crop))
-    check("conv5x5", inputs, 1e-4, wmask=wmask, relu=relu, residual=residual, crop=crop)
+            wmask = _safe_gate(O.conv5x5(*[t.double().to(dev) for t in inputs], relu=False, crop=crop)).cpu()
+    check("conv5x5", inputs, 1e-4, wmask=wmask, relu=relu, residual=residual, crop=crop, ref_device=dev)
 
 
 # --------------------------------------------------------------------------------------------------
