@@ -503,6 +503,7 @@ extern "C" int dfold_split2d(const float* x, long R, long C, long ld, int pre_re
         colsum_kernel<<<(unsigned)cdiv(C, 32), dim3(32, 32), 0, as_stream(stream)>>>(x, R, C, ld, pre_relu, gate, ldg, colsum);
         if (check_launch("colsum_kernel")) return 1;
     }
+    if (!hi && !hi_t) return 0;         // column sums only (a bias gradient without operand planes)
     if (hi && !hi_t && (ld & 3) == 0 && (ldo & 3) == 0 && (cpad & 3) == 0 && (!gate || (ldg & 3) == 0) &&
         ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(gate)) & 15) == 0 &&
         ((reinterpret_cast<uintptr_t>(hi) | reinterpret_cast<uintptr_t>(lo)) & 7) == 0) {
@@ -517,7 +518,9 @@ extern "C" int dfold_split2d(const float* x, long R, long C, long ld, int pre_re
 
 extern "C" int dfold_conv_weight_prep(const float* w, int O, int I, int T, uint16_t* f_hi, uint16_t* f_lo, long ldi,
                                       uint16_t* d_hi, uint16_t* d_lo, long ldo, void* stream) {
-    DFOLD_REQUIRE(O > 0 && I > 0 && T > 0 && T <= 64, "dfold_conv_weight_prep: bad shape");
+    // the CTA stages a 32 x 32 x T tile in 32 * (32 T + 1) * 4 B of shared memory: T = 56 takes 229,504 B, T = 57 would take
+    // 233,600 B, more than the 227 KB (232,448 B) a Hopper block can reserve
+    DFOLD_REQUIRE(O > 0 && I > 0 && T > 0 && T <= 56, "dfold_conv_weight_prep: bad shape (need O, I > 0 and 1 <= T <= 56)");
     DFOLD_REQUIRE(ldi >= I && (d_hi == nullptr || ldo >= O), "dfold_conv_weight_prep: bad leading dims");
     dim3 grid((unsigned)cdiv(I, 32), (unsigned)cdiv(O, 32));
     const size_t smem = (size_t)32 * (32 * T + 1) * sizeof(uint32_t);

@@ -41,14 +41,16 @@ int dfold_debug_gemm_stats(long long* buf);
  *   hi_t/lo_t : [C][ldt] (transposed), columns [R, rpad) zeroed   (nullable pair)
  * pre_relu applies max(x,0) first; gate (nullable, row stride ldg) zeroes x where gate <= 0 (ReLU backward);
  * colsum (nullable, [C], pre-zeroed) receives the column sums of the gated input (bias gradient), added in a fixed
- * order so that they are the same from run to run. */
+ * order so that they are the same from run to run.  With neither plane pair requested only the column sums run. */
 int dfold_split2d(const float* x, long R, long C, long ld, int pre_relu, const float* gate, long ldg,
                   uint16_t* hi, uint16_t* lo, long ldo, long cpad,
                   uint16_t* hi_t, uint16_t* lo_t, long ldt, long rpad, float* colsum, void* stream);
 
 /* Conv weight w[O][I][T] (the reference layout [C_out, C_in, 5, 5], T = 25) ->
  *   forward planes  f_hi/f_lo [T][O][ldi]           (K = input channel)
- *   dgrad planes    d_hi/d_lo [T][I][ldo], tap order flipped (nullable pair) */
+ *   dgrad planes    d_hi/d_lo [T][I][ldo], tap order flipped (nullable pair)
+ * 1 <= T <= 56: a CTA stages a 32 x 32 x T tile in shared memory.  Only columns [0, I) / [0, O) of each plane row are
+ * written; the caller zero-fills the padding up to ldi / ldo. */
 int dfold_conv_weight_prep(const float* w, int O, int I, int T, uint16_t* f_hi, uint16_t* f_lo, long ldi,
                            uint16_t* d_hi, uint16_t* d_lo, long ldo, void* stream);
 
