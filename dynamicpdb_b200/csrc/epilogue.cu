@@ -12,6 +12,7 @@
 //                              (rot_matmul, rot_vec_mul), :618-702 (Rotation.compose_r/apply/invert_apply),
 //                              :1065-1146 (Rigid.compose / apply / invert_apply / invert) and their autograd.
 #include "common.cuh"
+#include "igso3.cuh"
 
 namespace dfold {
 namespace {
@@ -53,17 +54,7 @@ struct ScoreParams {
 };
 
 __device__ __forceinline__ double sigma_of_t(const ScoreParams& p) {
-    const double t = *p.t;
-    const double s = log(t * p.e_max + (1.0 - t) * p.e_min);
-    // number of grid points <= s, minus one (np.digitize(..) - 1), clamped
-    int lo = 0, hi = p.G;
-    while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (p.grid[mid] <= s) lo = mid + 1; else hi = mid;
-    }
-    int idx = lo - 1;
-    idx = idx < 0 ? 0 : (idx >= p.G ? p.G - 1 : idx);
-    return p.grid[idx];
+    return p.grid[sigma_index(*p.t, p.grid, p.G, p.e_max, p.e_min)];
 }
 
 // everything between the two quaternions and the rotation vector, fp32 as in the reference (utils.py:589-606)
@@ -95,38 +86,6 @@ __device__ __forceinline__ RotVec rotvec_of(const Q4& qp, const Q4& qt, Q4& inv,
     return r;
 }
 
-// IGSO(3) series at angle omega (fp32 trigonometry of fp32 arguments, fp64 weights and sums: so3_diffuser.py:9-49,71-117)
-template <bool kSecond>
-__device__ __forceinline__ void igso3_series(float omega, double sigma, int L, int lane, double& S, double& dS, double& d2S) {
-    const float half_om = omega / 2.f;
-    const float lo = sinf(half_om);
-    const float dlo = 0.5f * cosf(half_om);
-    const float lo2 = __fmul_rn(lo, lo);
-    const double s2h = sigma * sigma * 0.5;
-    double s = 0.0, ds = 0.0, d2s = 0.0;
-    for (int l = lane; l < L; l += 32) {
-        const double ex = -(double)l * (double)(l + 1) * s2h;
-        if (ex < -746.0) break;                                   // exp() is exactly 0 from here on
-        const double decay = (double)(2 * l + 1) * exp(ex);
-        const float h = (float)l + 0.5f;
-        const float arg = __fmul_rn(omega, h);
-        float sh, ch;
-        sincosf(arg, &sh, &ch);
-        const float dhi = __fmul_rn(h, ch);
-        const float num = __fsub_rn(__fmul_rn(lo, dhi), __fmul_rn(sh, dlo));
-        s += decay * (double)sh / (double)lo;
-        ds += decay * (double)num / (double)lo2;
-        if (kSecond) {
-            const double dlo_d = (double)dlo, lo_d = (double)lo, hi_d = (double)sh;
-            const double d2hi = -(double)h * (double)h * hi_d, d2lo = -0.25 * lo_d;
-            d2s += decay * ((lo_d * d2hi - hi_d * d2lo) / (lo_d * lo_d) - 2.0 * dlo_d * (double)num / (lo_d * lo_d * lo_d));
-        }
-    }
-    S = warp_sum_d(s);
-    dS = warp_sum_d(ds);
-    d2S = kSecond ? warp_sum_d(d2s) : 0.0;
-}
-
 template <typename TT>
 __global__ void __launch_bounds__(256) score_fwd_kernel(const ScoreParams p, double* __restrict__ rot_score, TT* __restrict__ trans_score) {
     const long i = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -139,7 +98,7 @@ __global__ void __launch_bounds__(256) score_fwd_kernel(const ScoreParams p, dou
         const RotVec r = rotvec_of(ldq(p.q_pred + 4 * i), ldq(p.q_t + 4 * i), inv, n2);
         const float omega = r.vnorm + 1e-6f;
         double S, dS, d2S;
-        igso3_series<false>(omega, sigma, p.L, lane, S, dS, d2S);
+        igso3_series<float, false>(omega, sigma, p.L, lane, S, dS, d2S);
         if (lane < 3) {
             const double g = dS / (S + 1e-4);
             const float v = lane == 0 ? r.vx : (lane == 1 ? r.vy : r.vz);
@@ -173,7 +132,7 @@ __global__ void __launch_bounds__(256) score_bwd_kernel(const ScoreParams p, con
             const RotVec r = rotvec_of(qp, qt, inv, n2);
             const float omega = r.vnorm + 1e-6f;
             double S, dS, d2S;
-            igso3_series<true>(omega, sigma, p.L, lane, S, dS, d2S);
+            igso3_series<float, true>(omega, sigma, p.L, lane, S, dS, d2S);
             if (lane == 0) {
                 const double den = S + 1e-4;
                 const double g = dS / den;

@@ -13,10 +13,13 @@ cannot keep one GPU fed, let alone eight.  Here:
 * ``featurize_window`` computes ``rigids_0`` and the torsion features of a window with one kernel on the device
   (csrc/featurize.cu), from the fp32 coordinates of the ``frame_time`` selected frames only;
 * ``WindowPrefetcher`` overlaps the next window's slicing and host->device copy (side stream, pinned staging buffers)
-  with the current training step.
+  with the current training step;
+* given a diffuser (``score_epilogue.SE3ScoreDiffuser``), the same side stream also noises the window (:332-349):
+  in training ``t ~ U(min_t, 1)`` is drawn on the device and ``forward_marginal`` (csrc/diffuse.cu) adds ``t``,
+  ``rigids_t``, both scores and both score scalings; in evaluation ``t = 1`` and ``sample_ref`` gives ``rigids_t``.
+  No value goes back to the host, so a window is a complete training batch without per-window host work.
 
-The forward-marginal noising (``diffuser.forward_marginal``, :337-342) stays with the caller's diffuser, as the north star
-leaves the diffusion loop in Python.  Evaluation-only fields (``atom37_pos``, ``atom14_pos``, ``rigidgroups_0``,
+Evaluation-only fields (``atom37_pos``, ``atom14_pos``, ``rigidgroups_0``,
 ``residx_atom14_to_atom37``) are not produced.
 """
 import pickle
@@ -115,12 +118,22 @@ class WindowPrefetcher:
     """Iterates device-resident feature dicts, one protein window per item: while the consumer trains on window i, a worker
     thread slices window i+1 into pinned staging buffers and a side stream copies it to the device and featurises it."""
 
-    def __init__(self, store: TrajectoryStore, rows: Sequence[Tuple[str, str, str, str]], device, training: bool = True, depth: int = 2):
+    def __init__(self, store: TrajectoryStore, rows: Sequence[Tuple[str, str, str, str]], device, training: bool = True, depth: int = 2,
+                 diffuser=None, min_t: float = 0.01, generator: Optional[torch.Generator] = None):
+        """``diffuser`` (an ``SE3ScoreDiffuser``, optional) makes every item a noised training batch (see the module
+        docstring); ``min_t`` is the loader's ``data_conf.min_t``; ``generator`` (a CUDA generator on ``device``) feeds t
+        and the diffusion draws, default: the device's default generator."""
         dev = torch.device(device)
         if dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device())
         self.store, self.rows, self.device, self.training, self.depth = store, list(rows), dev, training, depth
+        self.diffuser, self.min_t, self.generator = diffuser, float(min_t), generator
+        if not 0.0 <= self.min_t <= 1.0:
+            raise ValueError(f"min_t={min_t} outside [0, 1]")
         self.stream = torch.cuda.Stream(device=self.device)
+        if diffuser is not None:
+            diffuser.tables(self.device)                    # built once, before the side stream reads them
+            self.stream.wait_stream(torch.cuda.current_stream(self.device))
         self._staging: Dict = {}
         self._slot: Dict[str, int] = {}
         self._events: list = []
@@ -160,11 +173,27 @@ class WindowPrefetcher:
                 "fixed_mask": torch.zeros(nf, atom37.shape[1], dtype=torch.float64, device=self.device),
                 "sc_ca_t": torch.zeros(nf, atom37.shape[1], 3, dtype=torch.float32, device=self.device),
             })
+            if self.diffuser is not None:
+                feats.update(self._noise(feats["rigids_0"]))
             ev = torch.cuda.Event()
             ev.record(self.stream)
         self._events.append(ev)
         del self._events[:-(self.depth + 2)]
         return feats, ev
+
+    def _noise(self, rigids_0: torch.Tensor) -> Dict[str, torch.Tensor]:
+        """Dfold_data_loader_dynamic.py:332-357 on the device: training t = rng.uniform(min_t, 1) and forward_marginal; eval
+        t = 1 and sample_ref of nf * N frames.  ``t`` is a [1] fp64 tensor (the loader's t, batched)."""
+        nf, N = rigids_0.shape[0], rigids_0.shape[1]
+        if self.training:
+            u = torch.rand(1, dtype=torch.float64, device=self.device, generator=self.generator)
+            t = self.min_t + (1.0 - self.min_t) * u
+            out = self.diffuser.forward_marginal(rigids_0, t, diffuse_mask=None, generator=self.generator)
+        else:
+            t = torch.ones(1, dtype=torch.float64, device=self.device)
+            out = self.diffuser.sample_ref(nf * N, frame_time=nf, generator=self.generator, device=self.device)
+        out["t"] = t
+        return out
 
     def __iter__(self) -> Iterator[Dict[str, torch.Tensor]]:
         import queue

@@ -63,6 +63,8 @@ _SIGS = {
     "dfold_quat_mul_bwd": "ppppplip",
     "dfold_rot_compose_fwd": "pppp" + "pp" + "liip",
     "dfold_rot_compose_bwd": "pppp" + "pp" + "pppp" + "liip",
+    "dfold_igso3_tables": "piiipp" + "p",
+    "dfold_forward_marginal": "ppppp" + "pppp" + "iiidddd" + "f" + "iii" + "ppppp" + "lp",
 }
 _CT = {"p": ctypes.c_void_p, "l": ctypes.c_long, "i": ctypes.c_int, "f": ctypes.c_float, "d": ctypes.c_double}
 
@@ -1282,3 +1284,45 @@ def reverse_step(q_t, x_t, rot_score, trans_score, z_rot, z_trans, mask, *, g_ro
                                         int(center), int(diffuse_rot), int(diffuse_trans), _ptr(q_out), _ptr(x_out), F_, N_, _stream()),
                "dfold_reverse_step")
     return q_out, x_out
+
+
+def igso3_tables(sigma_grid, num_omega: int, L: int = 1000):
+    """IGSO(3) tables of the reference's SO3Diffuser (so3_diffuser.py:132-180) for the fp64 ``sigma_grid`` [G] on its device:
+    (cdf [G, num_omega], score_scaling [G]), both fp64."""
+    _need_cuda(sigma_grid)
+    with torch.cuda.device(sigma_grid.device):
+        g = sigma_grid.to(torch.float64).contiguous()
+        G = g.numel()
+        cdf = torch.empty(G, num_omega, dtype=torch.float64, device=g.device)
+        scaling = torch.empty(G, dtype=torch.float64, device=g.device)
+        _check(lib().dfold_igso3_tables(_ptr(g), G, int(num_omega), int(L), _ptr(cdf), _ptr(scaling), _stream()), "dfold_igso3_tables")
+    return cdf, scaling
+
+
+def forward_marginal(rigids_0, z_axis, u, z_trans, mask, t64, grid, cdf, score_scaling, *, max_sigma, min_sigma, min_b, max_b,
+                     r3_scale, L=1000, diffuse_rot=True, diffuse_trans=True, ref_mode=False, n=None):
+    """Forward-marginal noising of frames on the device (csrc/diffuse.cu).  rigids_0 [n,7] fp32 (None with ``ref_mode``),
+    draws z_axis [n,3], u [n], z_trans [n,3] fp64, mask [n] or None, t64 a [1] fp64 device tensor.  Returns (rigids_t [n,7]
+    fp32, rot_score [n,3] fp64, trans_score [n,3] fp64, rot_scaling [] fp64, trans_scaling [] fp64); with ``ref_mode`` only
+    rigids_t is written (the others are None)."""
+    _need_cuda(rigids_0, z_axis, u, z_trans, mask, t64, grid, cdf, score_scaling)
+    dev = t64.device
+    with torch.cuda.device(dev):
+        r0 = _f32c(rigids_0.detach()) if rigids_0 is not None else None
+        n = r0.shape[0] if r0 is not None else int(n)
+        f64 = lambda x: x.detach().to(torch.float64).contiguous() if x is not None else None
+        za, uu, zt = f64(z_axis), f64(u), f64(z_trans)
+        mk = _f32c(mask.detach()) if mask is not None else None
+        rig = torch.empty(n, 7, dtype=torch.float32, device=dev)
+        rs = ts = rsc = tsc = None
+        if not ref_mode:
+            rs = torch.empty(n, 3, dtype=torch.float64, device=dev)
+            ts = torch.empty(n, 3, dtype=torch.float64, device=dev)
+            sc = torch.empty(2, dtype=torch.float64, device=dev)
+            rsc, tsc = sc[0], sc[1]
+        _check(lib().dfold_forward_marginal(_ptr(r0), _ptr(za), _ptr(uu), _ptr(zt), _ptr(mk), _ptr(t64), _ptr(grid), _ptr(cdf),
+                                            _ptr(score_scaling), grid.numel(), cdf.shape[1], int(L), float(max_sigma),
+                                            float(min_sigma), float(min_b), float(max_b), float(r3_scale), int(diffuse_rot),
+                                            int(diffuse_trans), int(ref_mode), _ptr(rig), _ptr(rs), _ptr(ts), _ptr(rsc), _ptr(tsc),
+                                            n, _stream()), "dfold_forward_marginal")
+    return rig, rs, ts, rsc, tsc

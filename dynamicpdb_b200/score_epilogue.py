@@ -22,8 +22,13 @@ class SE3ScoreDiffuser:
         self.min_sigma, self.max_sigma, self.num_sigma = so3.min_sigma, so3.max_sigma, so3.num_sigma
         self.min_b, self.max_b, self.coordinate_scaling = r3.min_b, r3.max_b, r3.coordinate_scaling
         self.L = 1000
+        self.num_omega = getattr(so3, "num_omega", 1000)
+        self.diffuse_rot = getattr(se3_conf, "diffuse_rot", True)
+        self.diffuse_trans = getattr(se3_conf, "diffuse_trans", True)
+        self.frame_time = getattr(se3_conf, "frame_time", None)
         self._grid_np = self._sigma_np(np.linspace(0.0, 1.0, self.num_sigma))      # discrete_sigma, so3_diffuser.py:183
         self._grid = {}
+        self._tables = {}
 
     @classmethod
     def from_reference(cls, diffuser):
@@ -35,9 +40,13 @@ class SE3ScoreDiffuser:
             if so3 is None or r3 is None or so3.use_cached_score or so3.schedule != "logarithmic":
                 return None
             from types import SimpleNamespace
+            se3 = getattr(diffuser, "_se3_conf", None)
             conf = SimpleNamespace(
-                so3=SimpleNamespace(min_sigma=so3.min_sigma, max_sigma=so3.max_sigma, num_sigma=so3.num_sigma),
-                r3=SimpleNamespace(min_b=r3.min_b, max_b=r3.max_b, coordinate_scaling=r3._r3_conf.coordinate_scaling))
+                so3=SimpleNamespace(min_sigma=so3.min_sigma, max_sigma=so3.max_sigma, num_sigma=so3.num_sigma,
+                                    num_omega=len(so3.discrete_omega)),
+                r3=SimpleNamespace(min_b=r3.min_b, max_b=r3.max_b, coordinate_scaling=r3._r3_conf.coordinate_scaling),
+                diffuse_rot=bool(getattr(diffuser, "_diffuse_rot", True)), diffuse_trans=bool(getattr(diffuser, "_diffuse_trans", True)),
+                frame_time=getattr(se3, "frame_time", None) if getattr(se3, "dynamics", False) else None)
             return cls(conf)
         except AttributeError:
             return None
@@ -46,6 +55,105 @@ class SE3ScoreDiffuser:
         if device not in self._grid:
             self._grid[device] = torch.from_numpy(self._grid_np).to(device)
         return self._grid[device]
+
+    def tables(self, device):
+        """IGSO(3) tables of the angle sampler (so3_diffuser.py:132-180), built on `device` by one kernel
+        (csrc/diffuse.cu `igso3_tables_kernel`) on first use: (cdf [num_sigma, num_omega], score_scaling [num_sigma]), fp64."""
+        device = torch.device(device)
+        if device.type == "cuda" and device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        if device not in self._tables:
+            self._tables[device] = K.igso3_tables(self.grid(device), self.num_omega, self.L)
+        return self._tables[device]
+
+    def _t64(self, t, device) -> torch.Tensor:
+        """[1] fp64 device tensor of t: a Python number is checked to lie in [0, 1] (so3_diffuser.py:194-195); a tensor is
+        used where it lives and never read back to the host."""
+        if torch.is_tensor(t):
+            return t.reshape(-1)[:1].to(torch.float64)
+        t = float(t)
+        if not 0.0 <= t <= 1.0:
+            raise ValueError(f"Invalid t={t}")
+        return torch.full((1,), t, dtype=torch.float64, device=device)
+
+    def score_scaling(self, t, device=None):
+        """(rot_score_scaling, trans_score_scaling) at time t as fp64 device scalars: so3 ``_score_scaling[t_to_idx(t)]``
+        (so3_diffuser.py:307-309) and r3 ``1 / sqrt(1 - exp(-beta(t)))`` (r3_diffuser.py:103-104); 1 for a part that is not
+        diffused (se3_diffuser.py:65-84)."""
+        dev = t.device if torch.is_tensor(t) else torch.device(device if device is not None else "cuda")
+        K._need_cuda(torch.empty(0, device=dev))
+        t64 = self._t64(t, dev)[0]
+        one = torch.ones((), dtype=torch.float64, device=dev)
+        rot = one
+        if self.diffuse_rot:
+            grid = self.grid(dev)
+            s = torch.log(t64 * float(np.exp(self.max_sigma)) + (1 - t64) * float(np.exp(self.min_sigma)))
+            idx = (torch.bucketize(s, grid, right=True) - 1).clamp(0, grid.numel() - 1)
+            rot = self.tables(dev)[1][idx]
+        beta = t64 * self.min_b + 0.5 * t64 * t64 * (self.max_b - self.min_b)
+        trans = 1.0 / torch.sqrt(1.0 - torch.exp(-beta)) if self.diffuse_trans else one
+        return rot, trans
+
+    def _draws(self, n: int, device, draws, generator, rot: bool, trans: bool):
+        """The three fp64 draw buffers in the reference's consumption order (so3 axis normals, so3 uniforms, r3 normals);
+        ``draws`` (dict z_axis / u / z_trans) injects them, else they come from ``generator`` on the device."""
+        if draws is not None:
+            get = lambda k, c: draws[k].to(device=device, dtype=torch.float64).reshape(n, *c) if draws.get(k) is not None else None
+            return get("z_axis", (3,)), get("u", ()), get("z_trans", (3,))
+        z_axis = torch.randn(n, 3, dtype=torch.float64, device=device, generator=generator) if rot else None
+        u = torch.rand(n, dtype=torch.float64, device=device, generator=generator) if rot else None
+        z_trans = torch.randn(n, 3, dtype=torch.float64, device=device, generator=generator) if trans else None
+        return z_axis, u, z_trans
+
+    def forward_marginal(self, rigids_0, t, diffuse_mask=None, as_tensor_7: bool = True, *, draws=None, generator=None):
+        """``SE3Diffuser.forward_marginal`` (se3_diffuser.py:47-110) by ONE kernel on the device of ``rigids_0`` (csrc/diffuse.cu
+        `forward_marginal_kernel`): no host round trip, no scipy.  ``rigids_0`` is a Rigid or a [..., N, 7] tensor; ``t`` a
+        Python number in [0, 1] or a device tensor (read on the device only, so a graph can feed it).  Returns the
+        reference's keys: rigids_t [..., N, 7] fp32 (a Rigid when not ``as_tensor_7``), rot_score / trans_score [..., N, 3]
+        fp64, rot_score_scaling / trans_score_scaling fp64 scalars.  Quaternions come out with w >= 0 (the reference's
+        eigen-decomposition leaves the sign arbitrary).  ``diffuse_mask`` [..., N] is 0/1: scores are multiplied by it,
+        translations blended, rotations of 0 entries kept.  The draws come from ``generator`` (torch CUDA generator; the
+        reference draws from numpy's global stream, so samples agree in distribution) unless ``draws`` injects them."""
+        r7 = rigids_0 if torch.is_tensor(rigids_0) else rigids_0.to_tensor_7()
+        K._need_cuda(r7)
+        dev = r7.device
+        lead = r7.shape[:-1]
+        n = int(np.prod(lead))
+        cdf, scaling = self.tables(dev)
+        za, u, zt = self._draws(n, dev, draws, generator, self.diffuse_rot, self.diffuse_trans)
+        mask = None
+        if diffuse_mask is not None:
+            mask = (diffuse_mask if torch.is_tensor(diffuse_mask) else torch.as_tensor(np.asarray(diffuse_mask))).to(dev).reshape(n)
+        rig, rs, ts, rsc, tsc = K.forward_marginal(
+            r7.reshape(n, 7), za, u, zt, mask, self._t64(t, dev), self.grid(dev), cdf, scaling, max_sigma=self.max_sigma,
+            min_sigma=self.min_sigma, min_b=self.min_b, max_b=self.max_b, r3_scale=self.coordinate_scaling, L=self.L,
+            diffuse_rot=self.diffuse_rot, diffuse_trans=self.diffuse_trans)
+        rig = rig.reshape(lead + (7,))
+        return {"rigids_t": rig if as_tensor_7 else ru.Rigid.from_tensor_7(rig),
+                "trans_score": ts.reshape(lead + (3,)), "rot_score": rs.reshape(lead + (3,)),
+                "trans_score_scaling": tsc, "rot_score_scaling": rsc}
+
+    def sample_ref(self, n_samples: int, impute=None, diffuse_mask=None, as_tensor_7: bool = False, *, frame_time=None,
+                   draws=None, generator=None, device=None):
+        """``SE3Diffuser.sample_ref`` (se3_diffuser.py:217-280) in the dynamics layout the trajectory loader uses
+        (Dfold_data_loader_dynamic.py:344-349): {'rigids_t': [frame_time, n_samples / frame_time, 7] fp32} on ``device``
+        (default: the current CUDA device), IGSO(3) rotations at t = 1 and N(0, I) / coordinate_scaling translations, one
+        kernel.  The imputation branch (``impute`` / ``diffuse_mask``) is not supported."""
+        if impute is not None or diffuse_mask is not None:
+            raise ValueError("sample_ref: impute / diffuse_mask (the non-dynamics branch) are not supported")
+        if not (self.diffuse_rot and self.diffuse_trans):
+            raise ValueError("Must provide imputation values.")
+        ft = frame_time if frame_time is not None else self.frame_time
+        if ft is None or n_samples % ft:
+            raise ValueError(f"sample_ref: n_samples={n_samples} is not a multiple of frame_time={ft}")
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        K._need_cuda(torch.empty(0, device=dev))
+        cdf, scaling = self.tables(dev)
+        za, u, zt = self._draws(n_samples, dev, draws, generator, True, True)
+        rig = K.forward_marginal(None, za, u, zt, None, self._t64(1.0, dev), self.grid(dev), cdf, scaling, max_sigma=self.max_sigma,
+                                 min_sigma=self.min_sigma, min_b=self.min_b, max_b=self.max_b, r3_scale=self.coordinate_scaling,
+                                 L=self.L, ref_mode=True, n=n_samples)[0]
+        return {"rigids_t": rig.reshape(ft, n_samples // ft, 7)}
 
     def fused_scores(self, rigids_t, rigids_pred, t, mask, ipa_coordinate_scaling: float):
         """Both masked scores of the trunk epilogue (ipa_pytorch_dynamic.py:883-897) in ONE kernel launch

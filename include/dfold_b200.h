@@ -275,6 +275,34 @@ int dfold_reverse_step(const float* q_t, const float* x_t, const double* rot_sco
                        float* q_out, float* x_out, long F, long N, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Forward diffusion of a training window (csrc/diffuse.cu): the noising step of the data loader
+ * (src/data/Dfold_data_loader_dynamic.py:332-349) on the device.
+ * ---------------------------------------------------------------------------------------------------------- */
+/* IGSO(3) inverse-cdf tables in fp64, one CTA per sigma row (src/data/so3_diffuser.py:132-180): for sigma_grid [num_sigma]
+ * (discrete_sigma) and omega_j = (j+1) pi / num_omega, cdf [num_sigma][num_omega] = cumsum(pdf) / num_omega * pi with
+ * pdf = igso3_expansion (:9-49, L terms) * (1 - cos omega) / pi, and score_scaling [num_sigma] = sqrt(|sum sn^2 pdf /
+ * sum pdf|) / sqrt(3) with sn the score norms of :71-117.  Sums run in a fixed order: equal inputs give equal bits.
+ * Needs (L + 2 num_omega) * 8 B <= 227 KB. */
+int dfold_igso3_tables(const double* sigma_grid, int num_sigma, int num_omega, int L, double* cdf, double* score_scaling,
+                       void* stream);
+/* SE3Diffuser.forward_marginal (src/data/se3_diffuser.py:47-110) of n = F*N frames, one warp per frame: rigids_0 [n,7]
+ * (w,x,y,z, trans) at time *t (device scalar) -> rigids_t [n,7] fp32 (unit quaternion with w >= 0), rot_score /
+ * trans_score [n,3] fp64, *rot_scaling / *trans_scaling (device scalars).  Rotation: so3_diffuser.py:215-251, :274-327
+ * (axis z_axis / |z_axis|, angle np.interp(u, cdf[sigma_idx(t)], omega), fp64 score with L terms, R_t = R_0 Exp(v));
+ * translation: r3_diffuser.py:81-104, :159-177 (VP-SDE marginal and score in scaled units, x_t returned unscaled).
+ * Draws are inputs: z_axis [n,3], u [n] in [0,1), z_trans [n,3], fp64.  mask [n] (0/1) or NULL: scores multiplied by it,
+ * translations blended, rotations of mask-0 frames copied from rigids_0 (se3_diffuser.py:86-101).  diffuse_rot /
+ * diffuse_trans = 0 keep that part of rigids_0 with zero score and scaling 1 (:65-84).  ref_mode != 0 is
+ * SE3Diffuser.sample_ref (:217-280) with the dynamics layout: identity rotation and x_0 = 0, trans = z_trans /
+ * r3_scale, rigids_0 / mask / scores / scalings unused.  No host reads: graph-capturable. */
+int dfold_forward_marginal(const float* rigids_0, const double* z_axis, const double* u, const double* z_trans,
+                           const float* mask, const double* t, const double* sigma_grid, const double* cdf,
+                           const double* score_scaling, int num_sigma, int num_omega, int L, double max_sigma,
+                           double min_sigma, double min_b, double max_b, float r3_scale, int diffuse_rot,
+                           int diffuse_trans, int ref_mode, float* rigids_t, double* rot_score, double* trans_score,
+                           double* rot_scaling, double* trans_scaling, long n, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Training loss (csrc/loss.cu), SURVEY.md 8 f3: value and gradients of Experiment.loss_fn after the model call
  * (train_DFOLD_dynamics.py:1206-1400; torsion term openfold/utils/loss.py:52-76) in one kernel.  All tensors fp64;
  * per-residue inputs are those of the LAST frame ([N,...]), the masks cover all nf frames, t / rot_scaling are device
