@@ -19,8 +19,9 @@ cannot keep one GPU fed, let alone eight.  Here:
   ``rigids_t``, both scores and both score scalings; in evaluation ``t = 1`` and ``sample_ref`` gives ``rigids_t``.
   No value goes back to the host, so a window is a complete training batch without per-window host work.
 
-Evaluation-only fields (``atom37_pos``, ``atom14_pos``, ``rigidgroups_0``,
-``residx_atom14_to_atom37``) are not produced.
+With ``targets=True`` each item also carries the evaluation targets ``atom37_pos`` / ``atom37_mask`` (fp64, as the
+loader returns them) for ``metrics.evaluate_window``.  The other evaluation-only fields (``atom14_pos``,
+``rigidgroups_0``, ``residx_atom14_to_atom37``) are not produced.
 """
 import pickle
 import threading
@@ -119,15 +120,17 @@ class WindowPrefetcher:
     thread slices window i+1 into pinned staging buffers and a side stream copies it to the device and featurises it."""
 
     def __init__(self, store: TrajectoryStore, rows: Sequence[Tuple[str, str, str, str]], device, training: bool = True, depth: int = 2,
-                 diffuser=None, min_t: float = 0.01, generator: Optional[torch.Generator] = None):
+                 diffuser=None, min_t: float = 0.01, generator: Optional[torch.Generator] = None, targets: bool = False):
         """``diffuser`` (an ``SE3ScoreDiffuser``, optional) makes every item a noised training batch (see the module
         docstring); ``min_t`` is the loader's ``data_conf.min_t``; ``generator`` (a CUDA generator on ``device``) feeds t
-        and the diffusion draws, default: the device's default generator."""
+        and the diffusion draws, default: the device's default generator.  ``targets`` adds the evaluation targets
+        ``atom37_pos`` [nf, N, 37, 3] and ``atom37_mask`` [nf, N, 37], fp64 as ``_process_csv_row`` returns them (:249-250),
+        which ``metrics.evaluate_window`` scores the sample against."""
         dev = torch.device(device)
         if dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device())
         self.store, self.rows, self.device, self.training, self.depth = store, list(rows), dev, training, depth
-        self.diffuser, self.min_t, self.generator = diffuser, float(min_t), generator
+        self.diffuser, self.min_t, self.generator, self.targets = diffuser, float(min_t), generator, bool(targets)
         if not 0.0 <= self.min_t <= 1.0:
             raise ValueError(f"min_t={min_t} outside [0, 1]")
         self.stream = torch.cuda.Stream(device=self.device)
@@ -163,7 +166,11 @@ class WindowPrefetcher:
         with torch.cuda.stream(self.stream):
             cp = lambda t: t.to(self.device, non_blocking=True)
             atom37 = cp(self._stage("atom37", ent["atom37"], sl))
-            feats = featurize_window(atom37, cp(ent["atom_mask"]), cp(ent["aatype"]))
+            atom_mask = cp(ent["atom_mask"])
+            feats = featurize_window(atom37, atom_mask, cp(ent["aatype"]))
+            if self.targets:
+                feats["atom37_pos"] = atom37.to(torch.float64)
+                feats["atom37_mask"] = atom_mask.to(torch.float64).unsqueeze(0).expand(nf, -1, -1)
             feats.update({
                 "aatype": cp(ent["aatype"]).unsqueeze(0).expand(nf, -1),
                 "seq_idx": cp(ent["residue_index"]).unsqueeze(0).expand(nf, -1),

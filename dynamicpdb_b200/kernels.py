@@ -65,6 +65,10 @@ _SIGS = {
     "dfold_rot_compose_bwd": "pppp" + "pp" + "pppp" + "liip",
     "dfold_igso3_tables": "piiipp" + "p",
     "dfold_forward_marginal": "ppppp" + "pppp" + "iiidddd" + "f" + "iii" + "ppppp" + "lp",
+    "dfold_rot_trans_error": "pipi" + "iii" + "pp",
+    "dfold_atom_errors": "pipipi" + "iiii" + "pp",
+    "dfold_superimpose": "pipi" + "ll" + "pill" + "i" + "ii" + "pppp" + "p",
+    "dfold_drmsd": "pipi" + "ll" + "pill" + "i" + "ii" + "pp" + "p",
 }
 _CT = {"p": ctypes.c_void_p, "l": ctypes.c_long, "i": ctypes.c_int, "f": ctypes.c_float, "d": ctypes.c_double}
 

@@ -333,6 +333,43 @@ int dfold_featurize_window(const float* pos, const float* atom_mask, const long*
 int dfold_adam_amsgrad(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, long n,
                        float* step, int tick, float lr, float beta1, float beta2, float eps, float grad_scale, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Evaluation metrics (csrc/metrics.cu), SURVEY.md 8 f6: the arithmetic of Experiment.eval_fn (train_DFOLD_dynamics.py:
+ * 765-928) and compute_validation_metrics_all (:99-154) on the device.  All arithmetic is fp64; each coordinate input
+ * is fp32 (flag 0) or fp64 (flag != 0) and is upcast exactly.  Sums run in a fixed order (equal inputs give equal bits);
+ * no host reads, so every call is graph-capturable.
+ * ---------------------------------------------------------------------------------------------------------- */
+/* Experiment._calc_rot_trans_error (:1549-1568) over src/toolbox/rot_trans_error.py:7-73: pred / gt [nf][N][7]
+ * (w,x,y,z, trans).  out [4][nf] = mean over residues of degrees(2 acos |clip(q_gt.q_pred)|) (both normalised), mean
+ * |t_gt - t_pred| over residues and xyz (no mask), and the same two with gt[ref_frame] broadcast in place of pred
+ * (the reference uses ref_frame = nf - 2).  Needs 0 <= ref_frame < nf. */
+int dfold_rot_trans_error(const void* pred, int pred_f64, const void* gt, int gt_f64, int nf, int N, int ref_frame, double* out,
+                          void* stream);
+/* Masked atom errors over pred / gt [nf][N][A][3], mask [nf][N][A] (A >= 2, CA at column 1).  out [6][nf] = MAE and MSE
+ * of eval_fn (:892-912; sum over the xyz-expanded mask, so 3 sum m, 0/0 = NaN), rmsd_all and rmsd_ca of
+ * compute_validation_metrics_all (:143-146; sqrt(sum (gt m - pred m)^2 / (sum m + 1e-4))), sum m and sum m over CA.
+ * drop_last_atom != 0 zeroes mask[nf-1][N-1][A-1], eval_fn's `atom_mask[-1, -1, -1] = 0.0` (:893). */
+int dfold_atom_errors(const void* pred, int pred_f64, const void* gt, int gt_f64, const void* mask, int mask_f64, int nf, int N,
+                      int A, int drop_last_atom, double* out, void* stream);
+/* Batched Kabsch: B point sets of P points, point i of set s at p[s * set_stride + i * point_stride + 0..2] in both
+ * `reference` and `coords` (point_stride >= 3), mask entries at mask[s * mask_set_stride + i * mask_point_stride].
+ * Finds the proper rotation R and t minimising sum w |R coords + t - reference|^2 (Bio SVDSuperimposer as eval_fn
+ * :898-909 and openfold/utils/superimposition.py:20-77 call it) with Horn's quaternion key matrix and fixed-sweep Jacobi,
+ * centroids and covariance in separate passes.  mask_mode 0: w = 1; 1: w = mask (selection); 2: both coordinate sets
+ * multiplied by the mask, w = 1 (compute_validation_metrics_all :113-150).  rmsd [B] = sqrt(sum w |R c + t - r|^2 /
+ * sum w), from the applied transform; rot [B][9] (row-major), trans [B][3] and out_coords [B][P][3] = R coords + t may
+ * be NULL.  An empty set (sum w = 0) gives rmsd NaN, R = I, t = 0 and out_coords = coords. */
+int dfold_superimpose(const void* reference, int reference_f64, const void* coords, int coords_f64, long set_stride,
+                      long point_stride, const void* mask, int mask_f64, long mask_set_stride, long mask_point_stride, int mask_mode,
+                      int B, int P, double* rmsd, double* rot, double* trans, double* out_coords, void* stream);
+/* openfold/utils/validation_metrics.py:17-36 drmsd of B structure pairs of N points (layout as dfold_superimpose):
+ * out [B] = sqrt(sum_ij (|s1_i - s1_j| - |s2_i - s2_j|)^2 m_i m_j / (n (n - 1))), n = min over the B sets of sum m (N
+ * without a mask; n <= 1 gives 0).  premul != 0 multiplies both structures by the mask first (compute_validation_metrics_all
+ * :113-125).  partial: workspace of B * T * T doubles, T = ceil(N / 64), one fixed-order sum per 64 x 64 tile; B <= 65535. */
+int dfold_drmsd(const void* s1, int s1_f64, const void* s2, int s2_f64, long set_stride, long point_stride, const void* mask,
+                int mask_f64, long mask_set_stride, long mask_point_stride, int premul, int B, int N, double* partial, double* out,
+                void* stream);
+
 #ifdef __cplusplus
 }
 #endif
