@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdfold_b200.so")
-SOURCES = ["simt.cu", "rigid.cu", "epilogue.cu", "diffuse.cu", "metrics.cu", "loss.cu", "featurize.cu", "ipa_attn.cu", "ipa_v2.cu", "ipa_fused.cu", "gemm_sm90.cu"]
+SOURCES = ["simt.cu", "rigid.cu", "epilogue.cu", "diffuse.cu", "metrics.cu", "rollout.cu", "loss.cu", "featurize.cu", "ipa_attn.cu", "ipa_v2.cu", "ipa_fused.cu", "gemm_sm90.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]

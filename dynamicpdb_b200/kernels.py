@@ -69,6 +69,7 @@ _SIGS = {
     "dfold_atom_errors": "pipipi" + "iiii" + "pp",
     "dfold_superimpose": "pipi" + "ll" + "pill" + "i" + "ii" + "pppp" + "p",
     "dfold_drmsd": "pipi" + "ll" + "pill" + "i" + "ii" + "pp" + "p",
+    "dfold_rollout_advance": "pppppp" + "iiii" + "p",
 }
 _CT = {"p": ctypes.c_void_p, "l": ctypes.c_long, "i": ctypes.c_int, "f": ctypes.c_float, "d": ctypes.c_double}
 
@@ -1330,3 +1331,35 @@ def forward_marginal(rigids_0, z_axis, u, z_trans, mask, t64, grid, cdf, score_s
                                             int(diffuse_trans), int(ref_mode), _ptr(rig), _ptr(rs), _ptr(ts), _ptr(rsc), _ptr(tsc),
                                             n, _stream()), "dfold_forward_marginal")
     return rig, rs, ts, rsc, tsc
+
+
+def rollout_advance(rigid_pred, atom37, rigids_0, rigid_traj, atom_traj, step):
+    """One step of the rollout's bookkeeping on the device (csrc/rollout.cu, eval_extension train_DFOLD_dynamics.py:993-996):
+    with s = step[0] in [0, L) writes rigid_traj[s] = rigid_pred[-1] and atom_traj[s] = atom37[-1], shifts rigids_0 in place to
+    cat(rigid_pred[1:], rigid_pred[-1:]) and advances step; with s outside [0, L) writes nothing.  rigid_pred [nf,N,7] and
+    atom37 [nf,N,A,3] fp32 (copied when not contiguous); rigids_0 [nf,N,7], rigid_traj [L,N,7], atom_traj [L,N,A,3] contiguous
+    fp32 and step a [1] int64 device tensor, all written in place.  Nothing is read back, so the call can be graph-captured."""
+    _need_cuda(rigid_pred, atom37, rigids_0, rigid_traj, atom_traj, step)
+    for name, t in (("rigid_pred", rigid_pred), ("atom37", atom37), ("rigids_0", rigids_0), ("rigid_traj", rigid_traj),
+                    ("atom_traj", atom_traj)):
+        if t.dtype != torch.float32:
+            raise ValueError(f"rollout_advance: {name} must be fp32, got {t.dtype}")
+    for name, t in (("rigids_0", rigids_0), ("rigid_traj", rigid_traj), ("atom_traj", atom_traj), ("step", step)):
+        if not t.is_contiguous():
+            raise ValueError(f"rollout_advance: {name} is written in place and must be contiguous")
+    if step.dtype != torch.int64 or step.numel() != 1:
+        raise ValueError(f"rollout_advance: step must be one int64, got {step.dtype} {tuple(step.shape)}")
+    if rigid_pred.dim() != 3 or rigid_pred.shape[-1] != 7 or rigids_0.shape != rigid_pred.shape:
+        raise ValueError(f"rollout_advance: need rigid_pred / rigids_0 [nf, N, 7] of one shape, got {tuple(rigid_pred.shape)} and "
+                         f"{tuple(rigids_0.shape)}")
+    nf, N = rigid_pred.shape[0], rigid_pred.shape[1]
+    if atom37.dim() != 4 or atom37.shape[:2] != (nf, N) or atom37.shape[-1] != 3:
+        raise ValueError(f"rollout_advance: atom37 {tuple(atom37.shape)} is not [{nf}, {N}, A, 3]")
+    A, L = atom37.shape[2], rigid_traj.shape[0]
+    if tuple(rigid_traj.shape) != (L, N, 7) or tuple(atom_traj.shape) != (L, N, A, 3):
+        raise ValueError(f"rollout_advance: need rigid_traj [L, {N}, 7] and atom_traj [L, {N}, {A}, 3], got "
+                         f"{tuple(rigid_traj.shape)} and {tuple(atom_traj.shape)}")
+    with torch.cuda.device(rigids_0.device):
+        rp, a37 = rigid_pred.detach().contiguous(), atom37.detach().contiguous()
+        _check(lib().dfold_rollout_advance(_ptr(rp), _ptr(a37), _ptr(rigids_0), _ptr(rigid_traj), _ptr(atom_traj), _ptr(step),
+                                           nf, N, A, L, _stream()), "dfold_rollout_advance")

@@ -222,17 +222,10 @@ _EVAL_WINDOW_KEYS = ("torsion_angles_sin_cos", "torsion_angles_mask", "node_repr
                      "force", "vel")
 
 
-def evaluate_window(sampler, window: Dict[str, torch.Tensor], num_t: int, min_t: float, noise_scale: float = 1.0):
-    """One protein of eval_fn (train_DFOLD_dynamics.py:813-912) on the device.  ``window`` is an evaluation item of
-    ``WindowPrefetcher(..., training=False, diffuser=..., targets=True)`` (``rigids_t`` from ``sample_ref``, plus
-    ``atom37_pos`` / ``atom37_mask``); ``sampler`` a ``DeviceReverseDiffusion``.  The sampler's inputs are built as eval_fn
-    builds them: ``res_mask`` ones, ``fixed_mask`` zeros, ``sc_ca_t`` zeros, ``seq_idx = arange(1, N + 1)`` (not the
-    residue index); the targets never enter the sampler's graph.  Runs ``sampler.sample_graphed`` and returns
-    ``window_metrics`` of its ``rigid_pred`` / ``prot_traj[0]`` -- device tensors; nothing is read back."""
-    missing = [k for k in _EVAL_WINDOW_KEYS + ("atom37_pos", "atom37_mask") if k not in window]
-    if missing:
-        raise ValueError(f"evaluate_window: the window lacks {missing} (WindowPrefetcher(training=False, diffuser=..., "
-                         "targets=True) provides them)")
+def eval_sampler_inputs(window: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+    """The sampler inputs eval_fn (train_DFOLD_dynamics.py:826-844) and eval_extension (:954-966) build from a window:
+    the window's own fields of ``_EVAL_WINDOW_KEYS`` (the same tensors, not copies) plus ``res_mask`` ones, ``fixed_mask``
+    zeros, ``sc_ca_t`` zeros and ``seq_idx = arange(1, N + 1)`` (not the residue index)."""
     nf, N = window["rigids_0"].shape[:2]
     dev = window["rigids_0"].device
     init = {k: window[k] for k in _EVAL_WINDOW_KEYS}
@@ -242,6 +235,19 @@ def evaluate_window(sampler, window: Dict[str, torch.Tensor], num_t: int, min_t:
         "seq_idx": torch.arange(1, N + 1, device=dev).unsqueeze(0).repeat(nf, 1),
         "sc_ca_t": torch.zeros(nf, N, 3, dtype=torch.float32, device=dev),
     })
-    out = sampler.sample_graphed(init, num_t, min_t, noise_scale)
+    return init
+
+
+def evaluate_window(sampler, window: Dict[str, torch.Tensor], num_t: int, min_t: float, noise_scale: float = 1.0):
+    """One protein of eval_fn (train_DFOLD_dynamics.py:813-912) on the device.  ``window`` is an evaluation item of
+    ``WindowPrefetcher(..., training=False, diffuser=..., targets=True)`` (``rigids_t`` from ``sample_ref``, plus
+    ``atom37_pos`` / ``atom37_mask``); ``sampler`` a ``DeviceReverseDiffusion``.  The sampler's inputs are built as eval_fn
+    builds them (``eval_sampler_inputs``); the targets never enter the sampler's graph.  Runs ``sampler.sample_graphed`` and
+    returns ``window_metrics`` of its ``rigid_pred`` / ``prot_traj[0]`` -- device tensors; nothing is read back."""
+    missing = [k for k in _EVAL_WINDOW_KEYS + ("atom37_pos", "atom37_mask") if k not in window]
+    if missing:
+        raise ValueError(f"evaluate_window: the window lacks {missing} (WindowPrefetcher(training=False, diffuser=..., "
+                         "targets=True) provides them)")
+    out = sampler.sample_graphed(eval_sampler_inputs(window), num_t, min_t, noise_scale)
     return window_metrics(out["rigid_pred"], out["prot_traj"][0], window["rigids_0"], window["atom37_pos"],
                           window["atom37_mask"])

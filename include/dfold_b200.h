@@ -370,6 +370,20 @@ int dfold_drmsd(const void* s1, int s1_f64, const void* s2, int s2_f64, long set
                 int mask_f64, long mask_set_stride, long mask_point_stride, int premul, int B, int N, double* partial, double* out,
                 void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Trajectory rollout (csrc/rollout.cu), SURVEY.md 8 f7: the per-step bookkeeping of Experiment.eval_extension
+ * (train_DFOLD_dynamics.py:931-1000) on the device.
+ * ---------------------------------------------------------------------------------------------------------- */
+/* One step of the rollout loop, replacing :993-996 (atom_traj.append(atom_pred[-1:]), rigid_traj.append(rigid_pred[-1:]),
+ * valid_feats['rigids_0'] = cat(rigid_pred[1:], rigid_pred[-1:])).  rigid_pred [nf][N][7] and atom37 [nf][N][A][3] are the
+ * network's prediction (fp32); rigids_0 [nf][N][7] is shifted in place; `step` is a DEVICE int64 counter s.  With
+ * 0 <= s < L: rigid_traj[s] ([L][N][7]) = rigid_pred[nf-1], atom_traj[s] ([L][N][A][3]) = atom37[nf-1], rigids_0[f] =
+ * rigid_pred[min(f+1, nf-1)], then s += 1; otherwise nothing is written.  One launch of one CTA, no host reads, so a
+ * captured graph of (forward, advance) replays every step.  Needs nf >= 2, N, A, L >= 1 and rigid_pred disjoint from
+ * rigids_0. */
+int dfold_rollout_advance(const float* rigid_pred, const float* atom37, float* rigids_0, float* rigid_traj, float* atom_traj,
+                          long long* step, int nf, int N, int A, int L, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
