@@ -6,6 +6,10 @@
 // (:1337-1339) and the normalisation by the number of non-empty frames (:1374-1375).  One CTA, fp64 throughout (the
 // reference's loader hands float64 targets, which promotes the whole expression), deterministic tree reductions.
 // The O((5N)^2) pair-distance tensors and the ground-truth backbone of :1316-1365 never reach final_loss and are not built.
+// Gradients follow torch's autograd at the non-smooth points too: a vector norm has gradient 0 at 0, so a zero-length
+// predicted torsion (sin, cos) keeps the direct term w / 1e-8 of u / (|u| + 1e-8), and a zero rotation score of a counted
+// residue keeps d axis / 1e-6 of the separate loss's axis term; torch.minimum splits a tie between the two torsion
+// targets evenly.
 #include "common.cuh"
 
 namespace dfold {
@@ -99,7 +103,9 @@ __global__ void __launch_bounds__(LT) loss_kernel(const LossParams p) {
     const double g2 = (trans < 100.0) ? 1.0 : 0.0;
     tor *= g2;
     const double fin = rot + trans + tor;
-    const double nrm = (double)p.nf / (s_cnt + 1e-10);       // the per-frame value is repeated nf times, then summed / count
+    // the per-frame value is repeated nf times, then summed / (count + 1e-10); the count is an integer tensor, so torch
+    // forms that denominator in fp32: exactly the count when it is >= 1, fp32(1e-10) when every frame is empty
+    const double nrm = (double)p.nf / (double)((float)s_cnt + 1e-10f);
     if (tid == 0) {
         p.out[0] = fin * nrm; p.out[1] = rot * nrm; p.out[2] = trans * nrm; p.out[3] = tor * nrm;
         p.out[4] = rot; p.out[5] = trans; p.out[6] = tor; p.out[7] = fin;
@@ -112,16 +118,16 @@ __global__ void __launch_bounds__(LT) loss_kernel(const LossParams p) {
         for (int c = 0; c < 3; ++c) { g[c] = p.gt_rot[3 * i + c]; q[c] = p.rs[3 * i + c] * dm; }
         if (p.separate) {
             const double ga = sqrt(g[0] * g[0] + g[1] * g[1] + g[2] * g[2]), qa = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
-            if (qa > 0) {
-                // angle term: d (ga - qa)^2 = -2 (ga - qa) q / qa;  axis term: a = q / (qa + e)
-                double dax[3], dot = 0;
+            // angle term: d (ga - qa)^2 = -2 (ga - qa) q / qa;  axis term: a = q / (qa + e).  At q = 0 the norm's gradient
+            // is 0 (torch's convention), which drops the angle term but leaves the axis term's direct part d a / 1e-6.
+            double dax[3], dot = 0;
 #pragma unroll
-                for (int c = 0; c < 3; ++c) { dax[c] = -2.0 * (g[c] / (ga + 1e-6) - q[c] / (qa + 1e-6)); dot += dax[c] * q[c]; }
+            for (int c = 0; c < 3; ++c) { dax[c] = -2.0 * (g[c] / (ga + 1e-6) - q[c] / (qa + 1e-6)); dot += dax[c] * q[c]; }
 #pragma unroll
-                for (int c = 0; c < 3; ++c) {
-                    dq[c] = -2.0 * (ga - qa) * q[c] / qa * lm * inv_s2 * k_rot
-                            + (dax[c] / (qa + 1e-6) - q[c] * dot / (qa * (qa + 1e-6) * (qa + 1e-6))) * lm * k_axis;
-                }
+            for (int c = 0; c < 3; ++c) {
+                dq[c] = (qa > 0) ? -2.0 * (ga - qa) * q[c] / qa * lm * inv_s2 * k_rot
+                                       + (dax[c] / (qa + 1e-6) - q[c] * dot / (qa * (qa + 1e-6) * (qa + 1e-6))) * lm * k_axis
+                                 : dax[c] / 1e-6 * lm * k_axis;
             }
         } else {
 #pragma unroll
@@ -138,10 +144,12 @@ __global__ void __launch_bounds__(LT) loss_kernel(const LossParams p) {
             const double gx = p.a_gt[(i * 7 + a) * 2], gy = p.a_gt[(i * 7 + a) * 2 + 1];
             const double hx = p.a_alt[(i * 7 + a) * 2], hy = p.a_alt[(i * 7 + a) * 2 + 1];
             const double d1 = (vx - gx) * (vx - gx) + (vy - gy) * (vy - gy), d2 = (vx - hx) * (vx - hx) + (vy - hy) * (vy - hy);
-            const bool first = d1 <= d2;
-            const double wx = 2.0 * (vx - (first ? gx : hx)), wy = 2.0 * (vy - (first ? gy : hy));
+            // d min(d1, d2) / d v; a tie splits the gradient evenly between both targets, as torch.minimum does
+            const double wx = d1 < d2 ? 2.0 * (vx - gx) : (d1 > d2 ? 2.0 * (vx - hx) : (vx - gx) + (vx - hx));
+            const double wy = d1 < d2 ? 2.0 * (vy - gy) : (d1 > d2 ? 2.0 * (vy - hy) : (vy - gy) + (vy - hy));
             const double k = p.a_mask[i * 7 + a] / tor_den * p.w_tor * g2 * nrm;
-            double dx = 0, dy = 0;
+            // v = u / (n + 1e-8): at u = 0 the norm's gradient is 0 (torch's convention) and only the direct term w / 1e-8 remains
+            double dx = wx / ne, dy = wy / ne;
             if (n > 0) {
                 const double dot = wx * ux + wy * uy;
                 dx = wx / ne - ux * dot / (n * ne * ne);

@@ -179,3 +179,33 @@ def loss_variant(name: str):
     if "shift" in v:
         out["rigids"][..., 4:] += v["shift"]
     return feats, out, v.get("separate_rot_loss", False)
+
+
+# edge cases of the loss (tests/golden/loss_edges.pt, oracle/make_loss_edges_golden.py), each an edit of one variant:
+#   zero_torsion_alt_gt   the zero-length predicted torsion [-1, 0, 0] with alternative == target (torsions 0-2 and chis
+#                         that are not pi-periodic): the reference's gradient there is w / 1e-8
+#   zero_torsion_alt_neg  the same torsion with alternative == -target: torch.minimum's tie split cancels it to 0
+#   zero_rot_score        separate loss, a counted residue whose predicted rotation score is exactly 0
+#   t_at_threshold        t == rot_loss_t_threshold: the rotation gate is a strict comparison
+#   last_frame_masked     every residue of the trained-on frame masked out; the normaliser counts the other frames
+#   all_masked            every residue of every frame masked out
+LOSS_EDGES = ("zero_torsion_alt_gt", "zero_torsion_alt_neg", "zero_rot_score", "t_at_threshold", "last_frame_masked", "all_masked")
+
+
+def loss_edge(name: str):
+    """(batch, model_out, separate_rot_loss) of one edge case."""
+    assert name in LOSS_EDGES, name
+    feats, out, separate = loss_variant("separate" if name == "zero_rot_score" else "plain")
+    if name == "zero_torsion_alt_gt":
+        feats["alt_torsion_angles_sin_cos"] = feats["torsion_angles_sin_cos"].clone()
+    elif name == "zero_torsion_alt_neg":
+        feats["alt_torsion_angles_sin_cos"][-1, 0, 0] = -feats["torsion_angles_sin_cos"][-1, 0, 0]
+    elif name == "zero_rot_score":
+        out["rot_score"][-1, 4] = 0.0
+    elif name == "t_at_threshold":
+        feats["t"] = torch.tensor([0.2], dtype=torch.float64)
+    elif name == "last_frame_masked":
+        feats["res_mask"][-1] = 0
+    else:
+        feats["res_mask"][:] = 0
+    return feats, out, separate
