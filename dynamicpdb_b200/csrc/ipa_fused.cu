@@ -551,7 +551,7 @@ extern "C" int dfold_debug_ipa_stats(long long* buf) {
 
 // Fused forward core.  Writes the point and pair columns of the concat buffer and the bf16 hi/lo probability planes; the
 // scalar-value columns [0, H*C) are left to dfold_gemm_bf16x3_batched over those planes.
-// Shapes: H = 8, Pq = 8, Pv = 12, Cp = 32 (DFOLDv2 preset A); other shapes use dfold_ipa_prob_fwd / dfold_ipa_attn_fwd.
+// Shapes: H = 8, Pq = 8, Pv = 12, Cp = 32 (DFOLDv2 preset A); other shapes use dfold_ipa_attn_fwd.
 extern "C" int dfold_ipa_fused_fwd(const float* logit0, const float* q_pts, const float* kv_pts, const float* pair,
                                    const float* quat, const float* trans, const float* mask, const float* gamma,
                                    uint16_t* p_hi, uint16_t* p_lo, long ldp,

@@ -474,7 +474,7 @@ __global__ void row_ln_bwd_kernel(const float* __restrict__ x, const float* __re
 using namespace dfold;
 
 extern "C" const char* dfold_last_error(void) { return g_err; }
-extern "C" int dfold_abi_version(void) { return 3; }
+extern "C" int dfold_abi_version(void) { return 4; }
 
 // id of the CUDA-graph capture `stream` is recording into (0 when the stream is not capturing).  The host side keys
 // its cached operand planes on it: planes built inside one capture must never be reused by another graph.

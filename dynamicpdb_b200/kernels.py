@@ -46,10 +46,8 @@ _SIGS = {
     "dfold_ipa_attn_fwd": "plplppplpppp" + "iiiiiiii" + "ff" + "ppp",
     "dfold_ipa_attn_bwd": "plplppplpppp" + "iiiiiiii" + "ff" + "ppp" + "ppppppppp" + "p",
     "dfold_ipa_pre_bwd": "pp" + "iiiiiii" + "pp" + "pppp" + "p",
-    "dfold_ipa_prob_fwd": "plppplpppp" + "ppl" + "iiiiiiii" + "ff" + "pp",
-    "dfold_ipa_pair_fwd": "plppplpppp" + "ppl" + "iiiiiiii" + "ff" + "pp",
     "dfold_ipa_fused_fwd": "pppppppp" + "ppl" + "iiiiiiii" + "ff" + "pp",
-    "dfold_ipa_ds_bwd": "plppplpppp" + "ppl" + "iiiiiiii" + "ff" + "pppppp" + "pppp" + "p",
+    "dfold_ipa_ds_bwd": "ppppl" + "iiiii" + "pppp" + "pp" + "p",
     "dfold_gemm_bf16x3_batched": "ppllll" + "liill" + "ppllll" + "llil" + "pllilf" + "p",
     "dfold_gemm_wgrad_bf16x3_batched": "pplllll" + "pplllll" + "lll" + "i" + "iiiil" + "pllf" + "p",
     "dfold_score_fwd": "ppppp" + "pidddd" + "ffpil" + "ppi" + "p",
@@ -98,8 +96,7 @@ def exported_symbols():
 
 
 # kernels launched per C-ABI call (bench.py reports the total as `gpu_launches`)
-_LAUNCHES_PER_CALL = {"dfold_global_layernorm_fwd": 3, "dfold_global_layernorm_bwd": 3, "dfold_ipa_attn_bwd": 4,
-                      "dfold_ipa_ds_bwd": 3}
+_LAUNCHES_PER_CALL = {"dfold_global_layernorm_fwd": 3, "dfold_global_layernorm_bwd": 3, "dfold_ipa_attn_bwd": 4}
 LAUNCH_COUNT = 0
 # When True (set by train_step.TrainStep around its step), weight gradients of the convolution are accumulated by the kernel
 # straight into the parameter's existing .grad buffer and autograd receives None: the ConvNet is shared by the four blocks
@@ -862,15 +859,9 @@ def _planes_rows(x2):
 
 
 class _IpaAttnTCFn(Function):
-    """Tensor-core decomposition of the IPA core (csrc/ipa_v2.cu + csrc/gemm_sm100.cu) for shared (frame-invariant)
-    q/k/v and pair tensors — the DFOLDv2 case.  Probabilities are materialised once as bf16 hi/lo planes."""
-
-    @staticmethod
-    def _v2args(logit0, q_pts, kv_pts, pair, quat, trans, mask, gamma, p_hi, p_lo, ldp, F_, N_, H_, C_, Pq, Pv, Cp, dfold, inf, eps):
-        l_fs = 0 if logit0.shape[0] == 1 else H_ * N_ * N_
-        p_fs = 0 if pair.shape[0] == 1 else N_ * N_ * Cp
-        return (_ptr(logit0), l_fs, _ptr(q_pts), _ptr(kv_pts), _ptr(pair), p_fs, _ptr(quat), _ptr(trans), _ptr(mask),
-                _ptr(gamma), _ptr(p_hi), _ptr(p_lo), ldp, F_, N_, H_, C_, Pq, Pv, Cp, int(dfold), inf, eps)
+    """Tensor-core decomposition of the IPA core (csrc/ipa_fused.cu + csrc/ipa_v2.cu + csrc/gemm_sm90.cu) for the preset-A
+    head geometry with shared (frame-invariant) q/k/v and pair tensors — the DFOLDv2 case.  Probabilities are materialised
+    once as bf16 hi/lo planes."""
 
     @staticmethod
     @_on_device
@@ -885,21 +876,16 @@ class _IpaAttnTCFn(Function):
         dev = q_pts.device
         n8 = _pad8(N_)
         cat = torch.empty((F_, N_, D), dtype=torch.float32, device=dev)
-        fused = _fused_fwd_ok(H_, Pq, Pv, Cp)
         # the probability planes feed the P V GEMM and the backward GEMMs
         p_hi = torch.empty((F_, H_, N_, n8), dtype=torch.int16, device=dev)
         p_lo = torch.empty((F_, H_, N_, n8), dtype=torch.int16, device=dev)
-        args = _IpaAttnTCFn._v2args(logit0, q_pts, kv_pts, pair, quat, trans, mask, gamma, p_hi, p_lo, n8, F_, N_, H_, C_, Pq, Pv, Cp, dfold, inf, eps)
         alg_bytes = 4.0 * (F_ * N_ * (H_ * (4 * C_ + 3 * (2 * Pq + Pv) + 8 * Pv + Cp) + 8) + N_ * N_ * (H_ + Cp))
         with _timed("ipa_fwd", alg_bytes):
-            if fused:
-                # one kernel: distances, exact softmax, pair + value-point aggregation, frame transform, P planes
-                _check(lib().dfold_ipa_fused_fwd(_ptr(logit0), _ptr(q_pts), _ptr(kv_pts), _ptr(pair), _ptr(quat), _ptr(trans),
-                                                 _ptr(mask), _ptr(gamma), _ptr(p_hi), _ptr(p_lo), n8,
-                                                 F_, N_, H_, C_, Pq, Pv, Cp, int(dfold), inf, eps, _ptr(cat), _stream()),
-                       "dfold_ipa_fused_fwd")
-            else:
-                _check(lib().dfold_ipa_prob_fwd(*args, _ptr(cat), _stream()), "dfold_ipa_prob_fwd")
+            # one kernel: distances, exact softmax, pair + value-point aggregation, frame transform, P planes
+            _check(lib().dfold_ipa_fused_fwd(_ptr(logit0), _ptr(q_pts), _ptr(kv_pts), _ptr(pair), _ptr(quat), _ptr(trans),
+                                             _ptr(mask), _ptr(gamma), _ptr(p_hi), _ptr(p_lo), n8,
+                                             F_, N_, H_, C_, Pq, Pv, Cp, int(dfold), inf, eps, _ptr(cat), _stream()),
+                   "dfold_ipa_fused_fwd")
             # O = P V  on the tensor cores, written into the o-columns of the concat buffer
             vt = kv[0, :, :, C_:].permute(1, 2, 0).reshape(H_ * C_, N_).contiguous()        # [H*C, N]
             vt_hi, vt_lo = _planes_rows(vt)
@@ -907,8 +893,6 @@ class _IpaAttnTCFn(Function):
                 _ptr(p_hi), _ptr(p_lo), F_ * H_, N_, N_, n8, F_ * H_, H_, 1, 0, N_,
                 _ptr(vt_hi), _ptr(vt_lo), H_, C_, N_, vt_hi.shape[1], 0, 0, 1, C_,
                 _ptr(cat), D, F_ * N_, H_, C_, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
-            if not fused:
-                _check(lib().dfold_ipa_pair_fwd(*args, _ptr(cat), _stream()), "dfold_ipa_pair_fwd")
         ctx.save_for_backward(logit0, kv, q_pts, kv_pts, pair, quat, trans, mask, gamma, cat, p_hi, p_lo)
         ctx.meta = (Pq, Pv, dfold, inf, eps)
         return cat
@@ -954,59 +938,56 @@ class _IpaAttnTCFn(Function):
         dS = new(F_, H_, N_, N_)
         dgamma_part = torch.zeros(H_, F_ * N_, dtype=torch.float32, device=dev)      # per-CTA partials, summed in order
         dq_pts, dkv_pts = new(*q_pts.shape), new(*kv_pts.shape)
-        args = _IpaAttnTCFn._v2args(logit0, q_pts, kv_pts, pair, quat, trans, mask, gamma, p_hi, p_lo, n8, F_, N_, H_, C_, Pq, Pv, Cp, dfold, inf, eps)
-        pts_gemm = PQ3 <= 31 and os.environ.get("DFOLD_IPA_PTS_GEMM", "1") != "0"
         # rows (f, h, i) of the value-point output gradient: operand of dV_pts below and of the value-point term of dP here
         dg = d_og.reshape(F_, N_, H_, PV3).permute(0, 2, 1, 3).reshape(F_ * H_ * N_, PV3).contiguous()
         dg_hi, dg_lo = _planes_rows(dg)
-        Tog = None
-        if Pq == 8 and os.environ.get("DFOLD_IPA_DS_V1", "0") != "1":
-            # d_og . v_pts on the tensor cores: Tog[(f,h,i), j] = sum_e dg[(f,h,i), e] v_pts[(f,h,j), e]
-            vp = kv_pts.reshape(F_, N_, H_, W)[..., PQ3:].permute(0, 2, 1, 3).reshape(F_ * H_ * N_, PV3).contiguous()
-            vp_hi, vp_lo = _planes_rows(vp)
-            Tog = new(F_ * H_ * N_, N_)
-            _check(lib().dfold_gemm_bf16x3_batched(
-                _ptr(dg_hi), _ptr(dg_lo), F_ * H_, N_, PV3, dg_hi.shape[1], F_ * H_, F_ * H_, 1, 0, PV3,
-                _ptr(vp_hi), _ptr(vp_lo), F_ * H_, N_, PV3, vp_hi.shape[1], 0, 0, 1, N_,
-                _ptr(Tog), N_, F_ * H_ * N_, 1, 0, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
-        _check(lib().dfold_ipa_ds_bwd(*args, _ptr(dcat), _ptr(d_og), _ptr(delta), _ptr(dP), _ptr(Tz), _ptr(Tog), _ptr(dS), _ptr(dgamma_part),
-                                      None if pts_gemm else _ptr(dq_pts), _ptr(dkv_pts), _stream()), "dfold_ipa_ds_bwd")
+        # d_og . v_pts on the tensor cores: Tog[(f,h,i), j] = sum_e dg[(f,h,i), e] v_pts[(f,h,j), e]
+        vp = kv_pts.reshape(F_, N_, H_, W)[..., PQ3:].permute(0, 2, 1, 3).reshape(F_ * H_ * N_, PV3).contiguous()
+        vp_hi, vp_lo = _planes_rows(vp)
+        Tog = new(F_ * H_ * N_, N_)
+        _check(lib().dfold_gemm_bf16x3_batched(
+            _ptr(dg_hi), _ptr(dg_lo), F_ * H_, N_, PV3, dg_hi.shape[1], F_ * H_, F_ * H_, 1, 0, PV3,
+            _ptr(vp_hi), _ptr(vp_lo), F_ * H_, N_, PV3, vp_hi.shape[1], 0, 0, 1, N_,
+            _ptr(Tog), N_, F_ * H_ * N_, 1, 0, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
+        _check(lib().dfold_ipa_ds_bwd(_ptr(q_pts), _ptr(kv_pts), _ptr(p_hi), _ptr(p_lo), n8, F_, N_, H_, Pq, Pv,
+                                      _ptr(delta), _ptr(dP), _ptr(Tz), _ptr(Tog), _ptr(dS), _ptr(dgamma_part), _stream()),
+               "dfold_ipa_ds_bwd")
         dgamma = dgamma_part.sum(1)
         del Tz
         del dP
         del Tog
-        if pts_gemm:
-            # Point gradients as two small tensor-core contractions over dS instead of the CUDA-core / LDS-bound pass:
-            #   dq_pts[i] = -gamma (q_i rowsum_i - sum_j dS_ij k_j),   dk_pts[j] = gamma (sum_i dS_ij q_i - colsum_j k_j)
-            # with a ones column appended to the point operands so the row / column sums fall out of the same products.
-            ds_hi, ds_lo = _planes_rows(dS.reshape(F_ * H_ * N_, N_))                                   # [F*H*N, n8]
-            kq = kv_pts.reshape(F_, N_, H_, W)[..., :PQ3]
-            kt = torch.zeros((F_, H_, 32, N_), dtype=torch.float32, device=dev)
-            kt[:, :, :PQ3] = kq.permute(0, 2, 3, 1)
-            kt[:, :, PQ3] = 1.0
-            kt_hi, kt_lo = _planes_rows(kt.reshape(F_ * H_ * 32, N_))                                   # [F*H*32, n8]
-            g1 = new(F_ * H_ * N_, 32)
-            _check(lib().dfold_gemm_bf16x3_batched(
-                _ptr(ds_hi), _ptr(ds_lo), F_ * H_, N_, N_, ds_hi.shape[1], F_ * H_, F_ * H_, 1, 0, N_,
-                _ptr(kt_hi), _ptr(kt_lo), F_ * H_, 32, N_, kt_hi.shape[1], 0, 0, 1, 32,
-                _ptr(g1), 32, F_ * H_ * N_, 1, 0, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
-            qn = torch.zeros((F_, H_, N_, 32), dtype=torch.float32, device=dev)
-            qh = q_pts.reshape(F_, N_, H_, PQ3).permute(0, 2, 1, 3)                                     # [F,H,N,24]
-            qn[..., :PQ3] = qh
-            qn[..., PQ3] = 1.0
-            qn_hi, qn_lo = _planes_rows(qn.reshape(F_ * H_ * N_, 32))
-            g2 = new(F_ * H_, N_, 32)
-            _check(lib().dfold_gemm_wgrad_bf16x3_batched(
-                _ptr(ds_hi), _ptr(ds_lo), N_, N_, F_ * H_, ds_hi.shape[1], N_ * ds_hi.shape[1],
-                _ptr(qn_hi), _ptr(qn_lo), 32, N_, F_ * H_, qn_hi.shape[1], N_ * qn_hi.shape[1],
-                32, 1, N_, F_ * H_, 0, 1, 0, 1, 0,
-                _ptr(g2), 32, N_ * 32, 1.0, _stream()), "dfold_gemm_wgrad_bf16x3_batched")
-            g1 = g1.reshape(F_, H_, N_, 32)
-            gam = gamma.reshape(1, H_, 1, 1)
-            dq = -gam * (qh * g1[..., PQ3:PQ3 + 1] - g1[..., :PQ3])
-            dq_pts.copy_(dq.permute(0, 2, 1, 3).reshape(q_pts.shape))
-            dk = gam * (g2[..., :PQ3].reshape(F_, H_, N_, PQ3) - g2[..., PQ3:PQ3 + 1].reshape(F_, H_, N_, 1) * kq.permute(0, 2, 1, 3))
-            dkv_pts.reshape(F_, N_, H_, W)[..., :PQ3] = dk.permute(0, 2, 1, 3)
+        # Point gradients as two small tensor-core contractions over dS:
+        #   dq_pts[i] = -gamma (q_i rowsum_i - sum_j dS_ij k_j),   dk_pts[j] = gamma (sum_i dS_ij q_i - colsum_j k_j)
+        # with a ones column appended to the point operands (3 Pq = 24 coordinates + 1, padded to 32 columns) so the
+        # row / column sums fall out of the same products.
+        ds_hi, ds_lo = _planes_rows(dS.reshape(F_ * H_ * N_, N_))                                   # [F*H*N, n8]
+        kq = kv_pts.reshape(F_, N_, H_, W)[..., :PQ3]
+        kt = torch.zeros((F_, H_, 32, N_), dtype=torch.float32, device=dev)
+        kt[:, :, :PQ3] = kq.permute(0, 2, 3, 1)
+        kt[:, :, PQ3] = 1.0
+        kt_hi, kt_lo = _planes_rows(kt.reshape(F_ * H_ * 32, N_))                                   # [F*H*32, n8]
+        g1 = new(F_ * H_ * N_, 32)
+        _check(lib().dfold_gemm_bf16x3_batched(
+            _ptr(ds_hi), _ptr(ds_lo), F_ * H_, N_, N_, ds_hi.shape[1], F_ * H_, F_ * H_, 1, 0, N_,
+            _ptr(kt_hi), _ptr(kt_lo), F_ * H_, 32, N_, kt_hi.shape[1], 0, 0, 1, 32,
+            _ptr(g1), 32, F_ * H_ * N_, 1, 0, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
+        qn = torch.zeros((F_, H_, N_, 32), dtype=torch.float32, device=dev)
+        qh = q_pts.reshape(F_, N_, H_, PQ3).permute(0, 2, 1, 3)                                     # [F,H,N,24]
+        qn[..., :PQ3] = qh
+        qn[..., PQ3] = 1.0
+        qn_hi, qn_lo = _planes_rows(qn.reshape(F_ * H_ * N_, 32))
+        g2 = new(F_ * H_, N_, 32)
+        _check(lib().dfold_gemm_wgrad_bf16x3_batched(
+            _ptr(ds_hi), _ptr(ds_lo), N_, N_, F_ * H_, ds_hi.shape[1], N_ * ds_hi.shape[1],
+            _ptr(qn_hi), _ptr(qn_lo), 32, N_, F_ * H_, qn_hi.shape[1], N_ * qn_hi.shape[1],
+            32, 1, N_, F_ * H_, 0, 1, 0, 1, 0,
+            _ptr(g2), 32, N_ * 32, 1.0, _stream()), "dfold_gemm_wgrad_bf16x3_batched")
+        g1 = g1.reshape(F_, H_, N_, 32)
+        gam = gamma.reshape(1, H_, 1, 1)
+        dq = -gam * (qh * g1[..., PQ3:PQ3 + 1] - g1[..., :PQ3])
+        dq_pts.copy_(dq.permute(0, 2, 1, 3).reshape(q_pts.shape))
+        dk = gam * (g2[..., :PQ3].reshape(F_, H_, N_, PQ3) - g2[..., PQ3:PQ3 + 1].reshape(F_, H_, N_, 1) * kq.permute(0, 2, 1, 3))
+        dkv_pts.reshape(F_, N_, H_, W)[..., :PQ3] = dk.permute(0, 2, 1, 3)
         # ---- dV[j,h,c] = sum_{f,i} P[f,h,i,j] dO[f,i,h,c]   (MN-major, K over all frames) ----
         dkv = torch.zeros_like(kv)
         _check(lib().dfold_gemm_wgrad_bf16x3_batched(
@@ -1033,26 +1014,22 @@ class _IpaAttnTCFn(Function):
         return dlogit0, dkv, dq_pts, dkv_pts, dpair, dquat, dtrans, None, dgamma, None, None, None, None, None
 
 
-def _fused_fwd_ok(H, Pq, Pv, Cp) -> bool:
-    """csrc/ipa_fused.cu is built for the DFOLDv2 preset-A head geometry; DFOLD_IPA_UNFUSED=1 keeps the three-kernel path."""
-    return H == 8 and Pq == 8 and Pv == 12 and Cp == 32 and os.environ.get("DFOLD_IPA_UNFUSED", "0") != "1"
-
-
 def _tc_path_ok(logit0, kv, q_pts, pair, Pq, Pv) -> bool:
-    """The tensor-core decomposition needs frame-shared q/k/v and pair tensors, a head width that is a whole number
-    of 64-wide K blocks, rows that fit in shared memory and point counts within its register tiles
-    (csrc/ipa_v2.cu v2_params: 3*Pq <= 48, 3*Pv <= 64)."""
+    """The tensor-core decomposition is built for the DFOLDv2 preset-A head geometry (H 8, Pq 8, Pv 12, Cp 32: the fused
+    forward csrc/ipa_fused.cu and the dS kernel csrc/ipa_v2.cu) and needs frame-shared q/k/v and pair tensors, a head
+    width that is a whole number of 64-wide K blocks and rows that fit in shared memory."""
     C_ = kv.shape[-1] // 2
-    N_ = q_pts.shape[1]
-    return (kv.shape[0] == 1 and pair.shape[0] == 1 and C_ % 64 == 0 and N_ <= 1280 and N_ % 8 == 0
-            and pair.shape[-1] % 8 == 0 and 3 * Pq <= 48 and 3 * Pv <= 64)
+    N_, H_ = q_pts.shape[1], q_pts.shape[2]
+    return (H_ == 8 and Pq == 8 and Pv == 12 and pair.shape[-1] == 32
+            and kv.shape[0] == 1 and pair.shape[0] == 1 and C_ % 64 == 0 and N_ <= 1280 and N_ % 8 == 0)
 
 
 def ipa_attention(logit0, kv, q_pts, kv_pts, pair, quat, trans, mask, gamma, *, Pq, Pv, dfold, inf, eps):
     """IPA core -> concat buffer [F,N,D] in the reference's feature order.
 
-    Frame-shared q/k/v with C % 64 == 0 (DFOLDv2, preset A) runs the tensor-core decomposition (csrc/ipa_v2.cu);
-    every other shape runs the single fused CUDA-core kernel (csrc/ipa_attn.cu).  Both are this library's kernels."""
+    The preset-A head geometry with frame-shared q/k/v, C % 64 == 0 and N <= 1280 (DFOLDv2) runs the tensor-core
+    decomposition (csrc/ipa_fused.cu, csrc/ipa_v2.cu); every other shape runs the single fused CUDA-core kernel
+    (csrc/ipa_attn.cu).  Both are this library's kernels."""
     if _tc_path_ok(logit0, kv, q_pts, pair, Pq, Pv):
         return _IpaAttnTCFn.apply(logit0, kv, q_pts, kv_pts, pair, quat, trans, mask, gamma, Pq, Pv, dfold, inf, eps)
     return _IpaAttnFn.apply(logit0, kv, q_pts, kv_pts, pair, quat, trans, mask, gamma, Pq, Pv, dfold, inf, eps)

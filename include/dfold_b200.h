@@ -176,19 +176,9 @@ int dfold_ipa_attn_bwd(const float* logit0, long logit0_fstride, const float* kv
                        float* dtrans, float* dgamma, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Tensor-core decomposition of the same IPA core (csrc/ipa_v2.cu): the probabilities are materialised once as
- * bf16 hi/lo planes P[F,H,N,ldp]; O = P V, dP, dV, dV_pts, dZ run on dfold_gemm_bf16x3*_batched.
+ * Tensor-core path for the preset-A head geometry (csrc/ipa_fused.cu, csrc/ipa_v2.cu): the probabilities are
+ * materialised once as bf16 hi/lo planes P[F,H,N,ldp]; O = P V, dP, dV, dV_pts, dZ run on dfold_gemm_bf16x3*_batched.
  * ---------------------------------------------------------------------------------------------------------- */
-/* logits + exact softmax -> P planes; aggregated value points, local-frame transform and norms -> concat buffer. */
-int dfold_ipa_prob_fwd(const float* logit0, long logit0_fstride, const float* q_pts, const float* kv_pts, const float* pair,
-                       long pair_fstride, const float* quat, const float* trans, const float* mask, const float* gamma,
-                       uint16_t* p_hi, uint16_t* p_lo, long ldp, int F, int N, int H, int C, int Pq, int Pv, int Cp,
-                       int dfold, float inf, float eps, float* out_cat, void* stream);
-/* o_pair[f,i,h,:] = sum_j P[f,h,i,j] z[i,j,:] -> pair columns of the concat buffer (ipa_pytorch_dynamic.py:498-502). */
-int dfold_ipa_pair_fwd(const float* logit0, long logit0_fstride, const float* q_pts, const float* kv_pts, const float* pair,
-                       long pair_fstride, const float* quat, const float* trans, const float* mask, const float* gamma,
-                       uint16_t* p_hi, uint16_t* p_lo, long ldp, int F, int N, int H, int C, int Pq, int Pv, int Cp,
-                       int dfold, float inf, float eps, float* out_cat, void* stream);
 /* Fused forward core (csrc/ipa_fused.cu), frame-shared logit0 [H,N,N] and pair [N,N,Cp]: one kernel does the point
  * distances (exact fp32), the exact two-pass softmax, the pair and value-point aggregations, the local-frame transform and
  * the concat layout; p_hi / p_lo receive the bf16 hi/lo probability planes, which feed the P V GEMM and the backward GEMMs:
@@ -204,18 +194,13 @@ int dfold_debug_ipa_stats(long long* buf);
 int dfold_ipa_pre_bwd(const float* quat, const float* trans, int F, int N, int H, int C, int Pv, int Cp, int dfold,
                       const float* out_cat, const float* dcat, float* d_og, float* delta, float* dquat, float* dtrans,
                       void* stream);
-/* dS = P (dP + d_og.v_pts + dO_pair.z - delta) [F,H,N,N], dgamma partials [H][F*N] as dfold_ipa_attn_bwd, dq_pts, key
- * part of dkv_pts.
- * Tz (nullable) = the dO_pair.z term precomputed as [N(i)][F*H][N(j)] by dfold_gemm_bf16x3_batched.
- * Tog (nullable; needs Tz and Pq = 8) = the value-point term d_og.v_pts precomputed as [F,H,N,N] the same way: the kernel then
- * keeps each key's points in registers and only adds, scales and accumulates d(gamma).  dq_pts null: the caller computes
- * the point gradients as contractions over dS. */
-int dfold_ipa_ds_bwd(const float* logit0, long logit0_fstride, const float* q_pts, const float* kv_pts, const float* pair,
-                     long pair_fstride, const float* quat, const float* trans, const float* mask, const float* gamma,
-                     uint16_t* p_hi, uint16_t* p_lo, long ldp, int F, int N, int H, int C, int Pq, int Pv, int Cp,
-                     int dfold, float inf, float eps, const float* dcat, const float* d_og, const float* delta,
-                     const float* dP, const float* Tz, const float* Tog, float* dS, float* dgamma, float* dq_pts,
-                     float* dkv_pts, void* stream);
+/* dS = P (dP + d_og.v_pts + dO_pair.z - delta) [F,H,N,N] and dgamma partials [H][F*N] as dfold_ipa_attn_bwd, for Pq = 8
+ * (Pv a multiple of 4); q_pts [F,N,H,Pq,3], kv_pts [F,N,H,Pq+Pv,3], p_hi / p_lo the forward's probability planes.
+ * Tz = the dO_pair.z term precomputed as [N(i)][F*H][N(j)] by dfold_gemm_bf16x3_batched; Tog = the value-point term
+ * d_og.v_pts precomputed as [F,H,N,N] the same way.  The caller computes the point gradients as contractions over dS. */
+int dfold_ipa_ds_bwd(const float* q_pts, const float* kv_pts, const uint16_t* p_hi, const uint16_t* p_lo, long ldp, int F,
+                     int N, int H, int Pq, int Pv, const float* delta, const float* dP, const float* Tz, const float* Tog,
+                     float* dS, float* dgamma, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Score epilogue (csrc/epilogue.cu), one warp per residue, no [n,L] temporaries, no host synchronisation.

@@ -1,6 +1,6 @@
 """Development probe: time of the IPA forward core (K.ipa_attention) at the benchmark shape with CUDA events on the launching
-stream: fully fused (training forward with probability planes / inference without), fused CUDA-core part + separate P V GEMM,
-and the three-kernel path.  python tests/devtools/dev_ipa_fwd.py [F N]"""
+stream: the fused kernel + P V GEMM, as a training forward (with probability planes kept for the backward) and as an
+inference forward.  python tests/devtools/dev_ipa_fwd.py [F N]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import torch
@@ -27,9 +27,7 @@ def run(train):
 
 
 outs = {}
-for name, unf, train in (("fused train       ", "0", True), ("fused infer       ", "0", False),
-                         ("three kernels     ", "1", True)):
-    os.environ["DFOLD_IPA_UNFUSED"] = unf
+for name, train in (("fused train", True), ("fused infer", False)):
     for _ in range(3):
         outs[name] = run(train)
     torch.cuda.synchronize()
@@ -42,7 +40,3 @@ for name, unf, train in (("fused train       ", "0", True), ("fused infer       
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / n
     print(f"{name}: {ms:.3f} ms/call  {alg / ms / 1e6:.0f} GB/s algorithmic ({alg / 1e6:.0f} MB)")
-ref = outs["three kernels     "]
-for k, v in outs.items():
-    d = (v - ref).abs()
-    print(f"max |{k} - three kernels| = {d.max().item():.3e}  (o columns {d[..., :H * C].max().item():.3e}; max |out| {ref.abs().max().item():.3e})")

@@ -116,7 +116,7 @@ def test_c_abi_exports_every_declared_symbol():
     for name in declared:
         assert isinstance(getattr(L, name), ctypes._CFuncPtr), name
     assert declared == set(kernels.exported_symbols())
-    assert L.dfold_abi_version() == 3
+    assert L.dfold_abi_version() == 4
 
 
 def test_ctypes_signatures_match_the_header():

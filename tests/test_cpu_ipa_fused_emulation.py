@@ -99,7 +99,7 @@ def test_two_pass_tiled_softmax_and_split_product_match_the_oracle():
 def test_point_gradients_as_contractions_with_a_ones_column():
     """The backward computes dq_pts / dk_pts as two contractions over dS with a ones column appended to the point operands
     (kernels._IpaAttnTCFn.backward): the row / column sums of dS fall out of the same products.  Checked against the direct
-    sum over coordinate differences (csrc/ipa_v2.cu ipa_pts_grad_kernel), with the split-bf16 product error included."""
+    sum over coordinate differences (as csrc/ipa_attn.cu computes them), with the split-bf16 product error included."""
     torch.manual_seed(1)
     N, PQ3, gam = 96, 24, 0.17
     q, k = torch.randn(N, PQ3) * 6 + 20.0, torch.randn(N, PQ3) * 6 + 20.0     # coordinates far from the origin: cancellation

@@ -113,7 +113,7 @@ def unit(*s, grad=True):
 
 
 def test_library_loads():
-    assert K.lib().dfold_abi_version() == 3
+    assert K.lib().dfold_abi_version() == 4
 
 
 @pytest.mark.parametrize("M,Kd,N", [(5, 3, 16), (70, 14, 32), (33, 7, 6), (256, 160, 6), (100, 128, 8), (4096, 7, 6), (3000, 14, 32)])
@@ -219,15 +219,16 @@ def _ipa_inputs(F, N, H, C, Pq, Pv, Cp, Fs, Fz, masked):
     (3, 256, 8, 256, 8, 12, 32, 1, 1, True),   # preset A, N = 256
     (1, 32, 8, 256, 8, 12, 32, 1, 1, True),    # fused kernel, exactly one key tile
     (2, 24, 8, 256, 8, 12, 32, 1, 1, True),    # fused kernel, one partial key tile
-    (2, 136, 4, 64, 4, 6, 16, 1, 1, False),    # tensor-core path, vanilla layout, N not a multiple of 64
+    (2, 136, 4, 64, 4, 6, 16, 1, 1, False),    # C % 64 == 0 outside the preset-A heads: csrc/ipa_attn.cu, vanilla layout
+    (2, 136, 8, 64, 8, 12, 32, 1, 1, False),    # tensor-core path, vanilla layout, C = 64, N not a multiple of 64
     (2, 33, 4, 16, 4, 8, 64, 2, 2, False),     # vanilla OpenFold, batched z and per-frame s
     (3, 70, 2, 8, 2, 3, 4, 3, 1, True),        # per-frame s, shared z, N not a multiple of the tiles
     (1, 1024, 8, 256, 8, 12, 32, 1, 1, True),  # preset A at the long-chain benchmark length
     (2, 1000, 8, 256, 8, 12, 32, 1, 1, True),  # N not a multiple of 32, 64 or 128
     (1, 1280, 8, 256, 8, 12, 32, 1, 1, True),  # the longest N of the tensor-core path
     (1, 1288, 8, 256, 8, 12, 32, 1, 1, True),  # the first N past it: csrc/ipa_attn.cu (shared memory independent of N)
-    (2, 72, 4, 64, 12, 6, 16, 1, 1, True),     # tensor-core path with 3 Pq > 31: point gradients in ipa_pts_grad_kernel
-    (1, 616, 4, 64, 4, 8, 64, 1, 1, True),     # non-fused, N (H + Cp) > 40960 floats: ipa_pair_fwd reads z unstaged
+    (2, 72, 4, 64, 12, 6, 16, 1, 1, True),     # C % 64 == 0 with Pq = 12 (36 query-point coordinates): csrc/ipa_attn.cu
+    (1, 616, 4, 64, 4, 8, 64, 1, 1, True),     # C % 64 == 0, N = 616 with Cp = 64: csrc/ipa_attn.cu
 ])
 @pytest.mark.parametrize("masked", [False, True])
 def test_ipa_attention(F, N, H, C, Pq, Pv, Cp, Fs, Fz, dfold, masked):
