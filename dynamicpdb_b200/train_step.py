@@ -12,7 +12,9 @@ comparable to the device time, so the step is:
   ``linear_rbf``) simply contribute zeros — the reason the reference needs ``find_unused_parameters=True``;
 * ``torch.cuda.graph`` captures the whole step (the C-ABI kernels are plain stream launches; TMA descriptors are
   by-value kernel arguments), replays have no Python / launch overhead;
-* if capture is not possible the same step runs eagerly (``graph=False`` or on capture failure).
+* if capture is not possible the same step runs eagerly (``graph=False`` or on capture failure);
+* ``state_dict()`` / ``load_state_dict()`` save and resume the weights and the Adam(amsgrad) state in the reference
+  trainer's checkpoint format, loading in place so the captured graph keeps running (checkpoint.py).
 """
 import copy
 import os
@@ -23,6 +25,7 @@ from typing import Callable, Dict, Optional
 import torch
 import torch.distributed as dist
 
+from . import checkpoint as _ckpt
 from . import kernels as _kernels
 
 
@@ -32,9 +35,9 @@ class TrainStep:
                  warmup: int = 3):
         self.net, self.loss_fn, self.world = net, loss_fn, world_size
         self.params = [p for p in net.parameters() if p.requires_grad]
+        self.layout = _ckpt.flat_layout(net)             # where each trained parameter sits in the flat buffers
         dev = self.params[0].device
-        total = sum(p.numel() for p in self.params)
-        padded = (total + 3) // 4 * 4                      # the fused optimizer runs float4-wide over the flat buffers
+        padded = self.layout.numel                         # padded to a multiple of 4: the fused optimizer runs float4-wide
         self.flat_grad = torch.zeros(padded, dtype=torch.float32, device=dev)
         # Adam(amsgrad) as the reference trainer (train_DFOLD_dynamics.py:412).  Default: ONE fused kernel over flat
         # parameter / gradient / moment buffers (csrc/simt.cu adam_amsgrad_kernel, step counter on the device); with
@@ -177,3 +180,55 @@ class TrainStep:
         else:
             self._eager()
         return self.loss
+
+    def _host_flat(self, tensors) -> torch.Tensor:
+        """Per-parameter device tensors (in self.params order) gathered into one host buffer of the flat layout."""
+        flat = torch.zeros(self.layout.numel, dtype=torch.float32)
+        with torch.no_grad():
+            for t, v in zip(tensors, (v for v in _ckpt.views(self.layout, flat) if v is not None)):
+                v.copy_(t)
+        return flat
+
+    def state_dict(self) -> Dict[str, object]:
+        """``{'model': net.state_dict() on the host, 'optimizer': torch.optim.Adam(net.parameters(), lr,
+        amsgrad=True).state_dict()}`` (checkpoint.py).  Each flat buffer is copied to the host once; the per-parameter
+        tensors are views of those copies."""
+        if self.opt is None:
+            flat = [t.cpu() for t in (self.flat_param, self.exp_avg, self.exp_avg_sq, self.max_exp_avg_sq)]
+            step = float(self.step_count)
+        else:
+            flat = [self._host_flat(self.params)] + [self._host_flat(self.opt.state[p][k] for p in self.params)
+                                                     for k in _ckpt.MOMENTS]
+            step = float(self.opt.state[self.params[0]]["step"])     # foreach Adam advances every parameter's step together
+        trained = {n: v for n, v in zip(self.layout.names, _ckpt.views(self.layout, flat[0])) if v is not None}
+        model = {k: trained[k] if k in trained else v.detach().cpu() for k, v in self.net.state_dict().items()}
+        return {"model": model, "optimizer": _ckpt.optimizer_state_dict(self.layout, *flat[1:], step, self.lr)}
+
+    def load_state_dict(self, sd: Dict[str, object]) -> None:
+        """Loads ``state_dict()``'s dict or a checkpoint of the reference trainer (``module.`` prefixes, a non-capturable
+        optimizer's CPU ``step``) IN PLACE: the captured graph holds pointers to the parameter, moment and step buffers,
+        and keeps replaying them.  No ``optimizer`` (or None) is a weights-only warm start with zero moments and step.
+        Everything is validated before the first write (checkpoint.check_state): a refused load raises ValueError and
+        leaves the step as it was.  Every data-parallel rank loads the same file, so no collective is needed."""
+        model, entries, step = _ckpt.check_state(sd, self.layout, {k: v.shape for k, v in self.net.state_dict().items()},
+                                                 self.lr)
+        moments = _ckpt.optimizer_to_flat(self.layout, entries)
+        trained = {n for n, o in zip(self.layout.names, self.layout.offsets) if o is not None}
+        with torch.no_grad():
+            if self.opt is None:
+                self.flat_param.copy_(_ckpt.model_to_flat(self.layout, model))
+                for buf, m in zip((self.exp_avg, self.exp_avg_sq, self.max_exp_avg_sq), moments):
+                    buf.copy_(m)
+                self.step_count.fill_(step)
+            else:
+                per = [[v for v in _ckpt.views(self.layout, m) if v is not None] for m in moments]
+                for j, p in enumerate(self.params):
+                    st = self.opt.state[p]
+                    for k, src in zip(_ckpt.MOMENTS, per):
+                        st[k].copy_(src[j])
+                    st["step"].fill_(step)
+            for k, v in self.net.state_dict().items():
+                if self.opt is not None or k not in trained:
+                    v.copy_(model[k])
+        _kernels.invalidate_weight_cache()          # no bf16 weight plane from before the load may be reused
+        torch.cuda.synchronize()
