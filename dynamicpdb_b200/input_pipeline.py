@@ -50,17 +50,10 @@ def featurize_window(atom37: torch.Tensor, atom_mask: torch.Tensor, aatype: torc
     alt = torch.empty_like(tor)
     tm = torch.empty(nf, N, 7, dtype=torch.float64, device=dev)
     with torch.cuda.device(dev):
-        K._check(K.lib().dfold_featurize_window(K._ptr(pos), K._ptr(am), K._ptr(aa), K._ptr(table("chi_atom_indices", dev)),
-                                                K._ptr(table("chi_angles_mask", dev)), K._ptr(table("chi_pi_periodic", dev)),
-                                                nf, N, K._ptr(rig), K._ptr(tor), K._ptr(alt), K._ptr(tm),
-                                                ctypes_stream(dev)), "dfold_featurize_window")
+        K.launch("dfold_featurize_window", pos, am, aa, table("chi_atom_indices", dev), table("chi_angles_mask", dev),
+                 table("chi_pi_periodic", dev), nf, N, rig, tor, alt, tm)
     return {"rigids_0": rig, "torsion_angles_sin_cos": tor, "alt_torsion_angles_sin_cos": alt, "torsion_angles_mask": tm,
             "res_mask": am[:, 1].to(torch.float64).unsqueeze(0).expand(nf, -1)}
-
-
-def ctypes_stream(dev):
-    import ctypes
-    return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 class TrajectoryStore:

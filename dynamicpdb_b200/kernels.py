@@ -4,6 +4,8 @@ Every function here launches hand-written sm_90a kernels through ctypes with raw
 current CUDA stream.  There is NO CPU path and no fallback to torch library kernels for the arithmetic: if the
 shared library is missing, or a tensor is not on a CUDA device, the ops raise.  (The tests exercise the host-side
 module logic on CPU by monkey-patching these names with the oracle — that seam lives in tests/, not here.)
+Every entry point that launches kernels is called through ``launch(name, *args)``, which passes tensors as device
+pointers, appends the current stream and raises with the library's message on failure.
 
 torch is used for: device memory (``torch.empty``), streams, autograd bookkeeping, and trivial view / elementwise
 glue (cat, slicing, SiLU on tiny tensors, masks).
@@ -106,11 +108,20 @@ GRAD_ACCUMULATE_INPLACE = False
 PROFILE = None
 
 
-def _check(rc: int, what: str):
+_PASS = frozenset((int, float, type(None), ctypes.c_void_p))
+
+
+def launch(name: str, *args):
+    """Call the launching entry point ``name`` with ``args`` and the current stream (its last parameter): a tensor passes
+    its data pointer, None NULL, and anything else (``_ptr`` values, ints, floats) goes as is to the ctypes signature."""
     global LAUNCH_COUNT
+    # the set lookup settles the common scalar types before the slower isinstance against torch.Tensor's metaclass:
+    # eager sampling is bound by the host cost of its launches
+    rc = getattr(lib(), name)(*[a if type(a) in _PASS else ctypes.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else a
+                                for a in args], _stream())
     if rc != 0:
-        raise RuntimeError(f"{what}: {lib().dfold_last_error().decode()}")
-    LAUNCH_COUNT += _LAUNCHES_PER_CALL.get(what, 1)
+        raise RuntimeError(f"{name}: {lib().dfold_last_error().decode()}")
+    LAUNCH_COUNT += _LAUNCHES_PER_CALL.get(name, 1)
 
 
 class _timed:
@@ -198,9 +209,9 @@ def _pad8(n: int) -> int:
 def _sgemm(A, a_off, a_rs, a_cs, a_bs, a_bs2, B, b_off, b_rs, b_cs, b_bs, b_bs2, C, c_off, c_rs, c_cs, c_bs, c_bs2,
            M, N, K, *, R=None, r_off=0, r_rs=0, r_cs=0, r_bs=0, r_bs2=0, bias=None, batch=1, batch2=1,
            alpha=1.0, beta=1.0, act=0, pre_relu=0):
-    _check(lib().dfold_sgemm(_ptr(A, a_off), a_rs, a_cs, a_bs, a_bs2, _ptr(B, b_off), b_rs, b_cs, b_bs, b_bs2,
-                             _ptr(C, c_off), c_rs, c_cs, c_bs, c_bs2, _ptr(R, r_off), r_rs, r_cs, r_bs, r_bs2,
-                             _ptr(bias), batch, batch2, M, N, K, alpha, beta, act, pre_relu, 1, _stream()), "dfold_sgemm")
+    launch("dfold_sgemm", _ptr(A, a_off), a_rs, a_cs, a_bs, a_bs2, _ptr(B, b_off), b_rs, b_cs, b_bs, b_bs2,
+           _ptr(C, c_off), c_rs, c_cs, c_bs, c_bs2, _ptr(R, r_off), r_rs, r_cs, r_bs, r_bs2,
+           bias, batch, batch2, M, N, K, alpha, beta, act, pre_relu, 1)
 
 
 def _split2d(x2: torch.Tensor, *, pre_relu=False, gate=None, want=True, want_t=False, colsum=None,
@@ -224,9 +235,8 @@ def _split2d(x2: torch.Tensor, *, pre_relu=False, gate=None, want=True, want_t=F
         else:
             hit, lot = t_out
             ldt, rp = t_ld, rpad
-    _check(lib().dfold_split2d(_ptr(x2), R, C, x2.stride(0), int(pre_relu), _ptr(gate), gate.stride(0) if gate is not None else 0,
-                               _ptr(hi), _ptr(lo), c8, c8, _ptr(hit, t_off), _ptr(lot, t_off), ldt, rp,
-                               _ptr(colsum), _stream()), "dfold_split2d")
+    launch("dfold_split2d", x2, R, C, x2.stride(0), int(pre_relu), gate, gate.stride(0) if gate is not None else 0,
+           hi, lo, c8, c8, _ptr(hit, t_off), _ptr(lot, t_off), ldt, rp, colsum)
     return (hi, lo), (hit, lot)
 
 
@@ -293,8 +303,7 @@ def _conv_planes(w: torch.Tensor):
         mk = lambda *s: torch.zeros(s, dtype=torch.int16, device=w.device)
         f_hi, f_lo, d_hi, d_lo = mk(T, O, i8), mk(T, O, i8), mk(T, I, o8), mk(T, I, o8)
         wc = _f32c(w.detach())     # keep the converted tensor alive until the launch is enqueued
-        _check(lib().dfold_conv_weight_prep(_ptr(wc), O, I, T, _ptr(f_hi), _ptr(f_lo), i8,
-                                            _ptr(d_hi), _ptr(d_lo), o8, _stream()), "dfold_conv_weight_prep")
+        launch("dfold_conv_weight_prep", wc, O, I, T, f_hi, f_lo, i8, d_hi, d_lo, o8)
         return f_hi, f_lo, d_hi, d_lo
     return _cache_get("conv", w, build)
 
@@ -303,26 +312,14 @@ def _gemm(a_hi, a_lo, F, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f, taps_n, out
           F_out=None, f_start=0):
     F_out = F if F_out is None else F_out
     with _timed("gemm_bf16x3", 2.0 * F_out * Nr * K * n_out * taps_f * taps_n, f"kmajor F{F_out} N{Nr} K{K} out{n_out} taps{taps_f * taps_n}"):
-        _gemm_launch(a_hi, a_lo, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f, taps_n, out, ldo, bias, residual, ldr,
-                     alpha, beta, act)
-
-
-def _gemm_launch(a_hi, a_lo, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f, taps_n, out, ldo, bias, residual, ldr,
-                 alpha, beta, act):
-    _check(lib().dfold_gemm_bf16x3(_ptr(a_hi), _ptr(a_lo), F, F_out, f_start, Nr, K, lda, _ptr(b_hi), _ptr(b_lo), n_out, ldb, taps_f, taps_n,
-                                   _ptr(out), ldo, _ptr(bias), _ptr(residual), ldr, alpha, beta, act, _stream()),
-           "dfold_gemm_bf16x3")
+        launch("dfold_gemm_bf16x3", a_hi, a_lo, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f, taps_n,
+               out, ldo, bias, residual, ldr, alpha, beta, act)
 
 
 def _gemm_wgrad(a, M, lda, b, Nn, ldb, F, Nr, taps_f, taps_n, out, ldo, Fb=None, b_f_add=0):
     Fb = F if Fb is None else Fb
     with _timed("gemm_bf16x3", 2.0 * F * Nr * M * Nn * taps_f * taps_n, f"wgrad F{F} N{Nr} M{M} n{Nn} taps{taps_f * taps_n}"):
-        _gemm_wgrad_launch(a, M, lda, b, Nn, ldb, F, Fb, b_f_add, Nr, taps_f, taps_n, out, ldo)
-
-
-def _gemm_wgrad_launch(a, M, lda, b, Nn, ldb, F, Fb, b_f_add, Nr, taps_f, taps_n, out, ldo):
-    _check(lib().dfold_gemm_wgrad_bf16x3(_ptr(a[0]), _ptr(a[1]), M, lda, _ptr(b[0]), _ptr(b[1]), Nn, ldb, F, Fb, b_f_add, Nr, taps_f, taps_n,
-                                         _ptr(out), ldo, 1.0, _stream()), "dfold_gemm_wgrad_bf16x3")
+        launch("dfold_gemm_wgrad_bf16x3", a[0], a[1], M, lda, b[0], b[1], Nn, ldb, F, Fb, b_f_add, Nr, taps_f, taps_n, out, ldo, 1.0)
 
 
 _ACT = {None: 0, "relu": 1}
@@ -483,10 +480,10 @@ class _Conv5x5Fn(Function):
             wp = ctx.w_param
             acc = wp.grad if (GRAD_ACCUMULATE_INPLACE and wp is not None) else None
             if acc is not None and acc.dtype == torch.float32 and acc.is_contiguous() and acc.shape == w.shape and acc.device == g.device:
-                _check(lib().dfold_taps_to_param(_ptr(taps), Co, Ci, kh * kw, _ptr(acc), 1, _stream()), "dfold_taps_to_param")
+                launch("dfold_taps_to_param", taps, Co, Ci, kh * kw, acc, 1)
             else:
                 dw = torch.empty((Co, Ci, kh, kw), dtype=torch.float32, device=g.device)
-                _check(lib().dfold_taps_to_param(_ptr(taps), Co, Ci, kh * kw, _ptr(dw), 0, _stream()), "dfold_taps_to_param")
+                launch("dfold_taps_to_param", taps, Co, Ci, kh * kw, dw, 0)
         return dx, dw, db, None, (dy if has_r else None), None
 
 
@@ -509,8 +506,7 @@ class _GlobalLNFn(Function):
         y = torch.empty_like(xc)
         stats = torch.empty(2, dtype=torch.float32, device=x.device)
         ws = torch.empty(2048 + 2, dtype=torch.float64, device=x.device)
-        _check(lib().dfold_global_layernorm_fwd(_ptr(xc), _ptr(y), _ptr(stats), _ptr(ws), xc.numel(), eps, int(silu), _stream()),
-               "dfold_global_layernorm_fwd")
+        launch("dfold_global_layernorm_fwd", xc, y, stats, ws, xc.numel(), eps, int(silu))
         ctx.save_for_backward(xc, stats)
         ctx.silu = silu
         return y
@@ -522,8 +518,7 @@ class _GlobalLNFn(Function):
         g = _f32c(dy)
         dx = torch.empty_like(xc)
         ws = torch.empty(2048 + 2, dtype=torch.float64, device=xc.device)
-        _check(lib().dfold_global_layernorm_bwd(_ptr(xc), _ptr(g), _ptr(stats), _ptr(ws), _ptr(dx), xc.numel(), int(ctx.silu), _stream()),
-               "dfold_global_layernorm_bwd")
+        launch("dfold_global_layernorm_bwd", xc, g, stats, ws, dx, xc.numel(), int(ctx.silu))
         return dx, None, None
 
 
@@ -542,8 +537,7 @@ class _RowLNFn(Function):
         y = torch.empty_like(x2)
         stats = torch.empty((x2.shape[0], 2), dtype=torch.float32, device=x.device)
         wc, bc = _f32c(w), _f32c(b)
-        _check(lib().dfold_row_layernorm_fwd(_ptr(x2), _ptr(wc), _ptr(bc), _ptr(y), _ptr(stats), x2.shape[0], C, eps, _stream()),
-               "dfold_row_layernorm_fwd")
+        launch("dfold_row_layernorm_fwd", x2, wc, bc, y, stats, x2.shape[0], C, eps)
         ctx.save_for_backward(x2, w, stats)
         ctx.shape = x.shape
         return y.reshape(x.shape)
@@ -558,8 +552,7 @@ class _RowLNFn(Function):
         dw = torch.zeros(C, dtype=torch.float32, device=x2.device)
         db = torch.zeros(C, dtype=torch.float32, device=x2.device)
         wc = _f32c(w)
-        _check(lib().dfold_row_layernorm_bwd(_ptr(x2), _ptr(wc), _ptr(g), _ptr(stats), _ptr(dx), _ptr(dw), _ptr(db), x2.shape[0], C, _stream()),
-               "dfold_row_layernorm_bwd")
+        launch("dfold_row_layernorm_bwd", x2, wc, g, stats, dx, dw, db, x2.shape[0], C)
         return dx.reshape(ctx.shape), dw, db, None
 
 
@@ -578,7 +571,7 @@ class _QuatToRotFn(Function):
         qc = _f32c(q)
         n = qc.numel() // 4
         R = torch.empty(qc.shape[:-1] + (3, 3), dtype=torch.float32, device=q.device)
-        _check(lib().dfold_quat_to_rot_fwd(_ptr(qc), _ptr(R), n, _stream()), "dfold_quat_to_rot_fwd")
+        launch("dfold_quat_to_rot_fwd", qc, R, n)
         ctx.save_for_backward(qc)
         return R
 
@@ -588,7 +581,7 @@ class _QuatToRotFn(Function):
         (qc,) = ctx.saved_tensors
         dq = torch.empty_like(qc)
         gR = _f32c(dR)
-        _check(lib().dfold_quat_to_rot_bwd(_ptr(qc), _ptr(gR), _ptr(dq), qc.numel() // 4, _stream()), "dfold_quat_to_rot_bwd")
+        launch("dfold_quat_to_rot_bwd", qc, gR, dq, qc.numel() // 4)
         return dq
 
 
@@ -608,8 +601,7 @@ class _RigidApplyFn(Function):
         m = pts.shape[2]
         out = torch.empty((F_, N_, m, 3), dtype=torch.float32, device=quat.device)
         fs = 0 if pts.shape[0] == 1 else N_ * m * 3
-        _check(lib().dfold_rigid_apply_fwd(_ptr(quat), _ptr(trans), _ptr(pts), fs, _ptr(out), F_, N_, m, int(inverse), _stream()),
-               "dfold_rigid_apply_fwd")
+        launch("dfold_rigid_apply_fwd", quat, trans, pts, fs, out, F_, N_, m, int(inverse))
         ctx.save_for_backward(quat, trans, pts)
         ctx.inverse = inverse
         return out
@@ -625,8 +617,7 @@ class _RigidApplyFn(Function):
         dq = torch.empty_like(quat)
         dt = torch.empty_like(trans)
         gout = _f32c(dout)
-        _check(lib().dfold_rigid_apply_bwd(_ptr(quat), _ptr(trans), _ptr(pts), fs, _ptr(gout), _ptr(dpts), _ptr(dq), _ptr(dt),
-                                           F_, N_, m, int(ctx.inverse), _stream()), "dfold_rigid_apply_bwd")
+        launch("dfold_rigid_apply_bwd", quat, trans, pts, fs, gout, dpts, dq, dt, F_, N_, m, int(ctx.inverse))
         if pts.shape[0] == 1 and F_ > 1:
             dpts = dpts.sum(0, keepdim=True)
         return dq, dt, dpts, None
@@ -681,8 +672,7 @@ class _ComposeFn(Function):
         mc = _f32c(mask.expand(quat.shape[:-1] + (1,))) if mask is not None else None
         n = qc.numel() // 4
         qo, to = torch.empty_like(qc), torch.empty_like(tc)
-        _check(lib().dfold_compose_q_update_fwd(_ptr(qc), _ptr(tc), _ptr(uc), _ptr(mc), _ptr(qo), _ptr(to), n, _stream()),
-               "dfold_compose_q_update_fwd")
+        launch("dfold_compose_q_update_fwd", qc, tc, uc, mc, qo, to, n)
         ctx.save_for_backward(qc, uc, mc)
         return qo, to
 
@@ -693,8 +683,7 @@ class _ComposeFn(Function):
         n = qc.numel() // 4
         dq, dt, du = torch.empty_like(qc), torch.empty(qc.shape[:-1] + (3,), dtype=torch.float32, device=qc.device), torch.empty_like(uc)
         gq, gt = _f32c(dqo), _f32c(dto)    # both must stay alive: two temporaries may otherwise share one block
-        _check(lib().dfold_compose_q_update_bwd(_ptr(qc), _ptr(uc), _ptr(mc), _ptr(gq), _ptr(gt), _ptr(dq), _ptr(dt),
-                                                _ptr(du), n, _stream()), "dfold_compose_q_update_bwd")
+        launch("dfold_compose_q_update_bwd", qc, uc, mc, gq, gt, dq, dt, du, n)
         return dq, dt, du, None
 
 
@@ -782,7 +771,7 @@ class _IpaAttnFn(Function):
         # plus the per-sample pair bias and pair values
         alg_bytes = 4.0 * (F_ * N_ * (H_ * (4 * C_ + 3 * (2 * Pq + Pv) + 8 * Pv + Cp) + 8) + N_ * N_ * (H_ + Cp))
         with _timed("ipa_fwd", alg_bytes):
-            _check(lib().dfold_ipa_attn_fwd(*args, _ptr(cat), _ptr(lse), _stream()), "dfold_ipa_attn_fwd")
+            launch("dfold_ipa_attn_fwd", *args, cat, lse)
         ctx.save_for_backward(logit0, kv, q_pts, kv_pts, pair, quat, trans, mask, gamma, cat, lse)
         ctx.meta = (Pq, Pv, dfold, inf, eps)
         return cat
@@ -792,8 +781,8 @@ class _IpaAttnFn(Function):
         l_fs = 0 if logit0.shape[0] == 1 else H_ * N_ * N_
         kv_fs = 0 if kv.shape[0] == 1 else N_ * H_ * 2 * C_
         p_fs = 0 if pair.shape[0] == 1 else N_ * N_ * Cp
-        return (_ptr(logit0), l_fs, _ptr(kv), kv_fs, _ptr(q_pts), _ptr(kv_pts), _ptr(pair), p_fs, _ptr(quat), _ptr(trans),
-                _ptr(mask), _ptr(gamma), F_, N_, H_, C_, Pq, Pv, Cp, int(dfold), inf, eps)
+        return (logit0, l_fs, kv, kv_fs, q_pts, kv_pts, pair, p_fs, quat, trans, mask, gamma, F_, N_, H_, C_, Pq, Pv, Cp, int(dfold),
+                inf, eps)
 
     @staticmethod
     @_on_device
@@ -814,9 +803,7 @@ class _IpaAttnFn(Function):
         dquat, dtrans = new(*quat.shape), new(*trans.shape)
         dgamma_part = torch.zeros(H_, F_ * N_, dtype=torch.float32, device=dev)      # per-CTA partials, summed in order
         args = _IpaAttnFn._args(logit0, kv, q_pts, kv_pts, pair, quat, trans, mask, gamma, F_, N_, H_, C_, Pq, Pv, Cp, dfold, inf, eps)
-        _check(lib().dfold_ipa_attn_bwd(*args, _ptr(cat), _ptr(lse), _ptr(dcat), _ptr(d_og), _ptr(delta), _ptr(Pm), _ptr(dS),
-                                        _ptr(dq_pts), _ptr(dkv_pts), _ptr(dquat), _ptr(dtrans), _ptr(dgamma_part), _stream()),
-               "dfold_ipa_attn_bwd")
+        launch("dfold_ipa_attn_bwd", *args, cat, lse, dcat, d_og, delta, Pm, dS, dq_pts, dkv_pts, dquat, dtrans, dgamma_part)
         dgamma = dgamma_part.sum(1)
         NN = N_ * N_
         # ---- value gradient  dv[j,h,c] = sum_{f,i} P[h,f,i,j] dO[f,i,h,c] ----
@@ -882,17 +869,15 @@ class _IpaAttnTCFn(Function):
         alg_bytes = 4.0 * (F_ * N_ * (H_ * (4 * C_ + 3 * (2 * Pq + Pv) + 8 * Pv + Cp) + 8) + N_ * N_ * (H_ + Cp))
         with _timed("ipa_fwd", alg_bytes):
             # one kernel: distances, exact softmax, pair + value-point aggregation, frame transform, P planes
-            _check(lib().dfold_ipa_fused_fwd(_ptr(logit0), _ptr(q_pts), _ptr(kv_pts), _ptr(pair), _ptr(quat), _ptr(trans),
-                                             _ptr(mask), _ptr(gamma), _ptr(p_hi), _ptr(p_lo), n8,
-                                             F_, N_, H_, C_, Pq, Pv, Cp, int(dfold), inf, eps, _ptr(cat), _stream()),
-                   "dfold_ipa_fused_fwd")
+            launch("dfold_ipa_fused_fwd", logit0, q_pts, kv_pts, pair, quat, trans, mask, gamma, p_hi, p_lo, n8,
+                   F_, N_, H_, C_, Pq, Pv, Cp, int(dfold), inf, eps, cat)
             # O = P V  on the tensor cores, written into the o-columns of the concat buffer
             vt = kv[0, :, :, C_:].permute(1, 2, 0).reshape(H_ * C_, N_).contiguous()        # [H*C, N]
             vt_hi, vt_lo = _planes_rows(vt)
-            _check(lib().dfold_gemm_bf16x3_batched(
-                _ptr(p_hi), _ptr(p_lo), F_ * H_, N_, N_, n8, F_ * H_, H_, 1, 0, N_,
-                _ptr(vt_hi), _ptr(vt_lo), H_, C_, N_, vt_hi.shape[1], 0, 0, 1, C_,
-                _ptr(cat), D, F_ * N_, H_, C_, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
+            launch("dfold_gemm_bf16x3_batched",
+                   p_hi, p_lo, F_ * H_, N_, N_, n8, F_ * H_, H_, 1, 0, N_,
+                   vt_hi, vt_lo, H_, C_, N_, vt_hi.shape[1], 0, 0, 1, C_,
+                   cat, D, F_ * N_, H_, C_, 1.0)
         ctx.save_for_backward(logit0, kv, q_pts, kv_pts, pair, quat, trans, mask, gamma, cat, p_hi, p_lo)
         ctx.meta = (Pq, Pv, dfold, inf, eps)
         return cat
@@ -914,26 +899,25 @@ class _IpaAttnTCFn(Function):
         new = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
         d_og, delta = new(F_, N_, H_, Pv, 3), new(F_, H_, N_)
         dquat, dtrans = new(*quat.shape), new(*trans.shape)
-        _check(lib().dfold_ipa_pre_bwd(_ptr(quat), _ptr(trans), F_, N_, H_, C_, Pv, Cp, int(dfold), _ptr(cat), _ptr(dcat),
-                                       _ptr(d_og), _ptr(delta), _ptr(dquat), _ptr(dtrans), _stream()), "dfold_ipa_pre_bwd")
+        launch("dfold_ipa_pre_bwd", quat, trans, F_, N_, H_, C_, Pv, Cp, int(dfold), cat, dcat, d_og, delta, dquat, dtrans)
         # ---- dP = dO V^T  (batched over (f, h); K = the head's C columns of dO) ----
         dc_hi, dc_lo = _planes_rows(dcat.reshape(F_ * N_, D))                       # [F*N, D8]
         kv_hi, kv_lo = _planes_rows(kv.reshape(N_, H_ * 2 * C_))                    # [N, H*2C]
         dP = new(F_, H_, N_, N_)
-        _check(lib().dfold_gemm_bf16x3_batched(
-            _ptr(dc_hi), _ptr(dc_lo), F_, N_, D, dc_hi.shape[1], F_ * H_, H_, H_, C_, C_,
-            _ptr(kv_hi), _ptr(kv_lo), 1, N_, H_ * 2 * C_, kv_hi.shape[1], C_, 2 * C_, 0, N_,
-            _ptr(dP), N_, F_ * H_ * N_, 1, 0, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
+        launch("dfold_gemm_bf16x3_batched",
+               dc_hi, dc_lo, F_, N_, D, dc_hi.shape[1], F_ * H_, H_, H_, C_, C_,
+               kv_hi, kv_lo, 1, N_, H_ * 2 * C_, kv_hi.shape[1], C_, 2 * C_, 0, N_,
+               dP, N_, F_ * H_ * N_, 1, 0, 1.0)
         # ---- pair term of dP on the tensor cores:  Tz[i][f*H+h][j] = sum_c dOpair[f,i,h,c] z[i,j,c]  (batched over i) ----
         offPair = H_ * C_ + 4 * H_ * Pv
         dop = dcat[..., offPair:offPair + H_ * Cp].reshape(F_, N_, H_, Cp).permute(1, 0, 2, 3).reshape(N_ * F_ * H_, Cp).contiguous()
         do_hi, do_lo = _planes_rows(dop)                                           # [N*F*H, Cp8]  rows (i, f, h)
         z_hi, z_lo = _planes_rows(pair.reshape(N_ * N_, Cp))                       # [N*N, Cp8]    rows (i, j)
         Tz = new(N_, F_ * H_, N_)
-        _check(lib().dfold_gemm_bf16x3_batched(
-            _ptr(do_hi), _ptr(do_lo), N_, F_ * H_, Cp, do_hi.shape[1], N_, N_, 1, 0, Cp,
-            _ptr(z_hi), _ptr(z_lo), N_, N_, Cp, z_hi.shape[1], 0, 0, 1, N_,
-            _ptr(Tz), N_, N_ * F_ * H_, 1, 0, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
+        launch("dfold_gemm_bf16x3_batched",
+               do_hi, do_lo, N_, F_ * H_, Cp, do_hi.shape[1], N_, N_, 1, 0, Cp,
+               z_hi, z_lo, N_, N_, Cp, z_hi.shape[1], 0, 0, 1, N_,
+               Tz, N_, N_ * F_ * H_, 1, 0, 1.0)
         # ---- dS, d(gamma), point gradients ----
         dS = new(F_, H_, N_, N_)
         dgamma_part = torch.zeros(H_, F_ * N_, dtype=torch.float32, device=dev)      # per-CTA partials, summed in order
@@ -945,13 +929,11 @@ class _IpaAttnTCFn(Function):
         vp = kv_pts.reshape(F_, N_, H_, W)[..., PQ3:].permute(0, 2, 1, 3).reshape(F_ * H_ * N_, PV3).contiguous()
         vp_hi, vp_lo = _planes_rows(vp)
         Tog = new(F_ * H_ * N_, N_)
-        _check(lib().dfold_gemm_bf16x3_batched(
-            _ptr(dg_hi), _ptr(dg_lo), F_ * H_, N_, PV3, dg_hi.shape[1], F_ * H_, F_ * H_, 1, 0, PV3,
-            _ptr(vp_hi), _ptr(vp_lo), F_ * H_, N_, PV3, vp_hi.shape[1], 0, 0, 1, N_,
-            _ptr(Tog), N_, F_ * H_ * N_, 1, 0, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
-        _check(lib().dfold_ipa_ds_bwd(_ptr(q_pts), _ptr(kv_pts), _ptr(p_hi), _ptr(p_lo), n8, F_, N_, H_, Pq, Pv,
-                                      _ptr(delta), _ptr(dP), _ptr(Tz), _ptr(Tog), _ptr(dS), _ptr(dgamma_part), _stream()),
-               "dfold_ipa_ds_bwd")
+        launch("dfold_gemm_bf16x3_batched",
+               dg_hi, dg_lo, F_ * H_, N_, PV3, dg_hi.shape[1], F_ * H_, F_ * H_, 1, 0, PV3,
+               vp_hi, vp_lo, F_ * H_, N_, PV3, vp_hi.shape[1], 0, 0, 1, N_,
+               Tog, N_, F_ * H_ * N_, 1, 0, 1.0)
+        launch("dfold_ipa_ds_bwd", q_pts, kv_pts, p_hi, p_lo, n8, F_, N_, H_, Pq, Pv, delta, dP, Tz, Tog, dS, dgamma_part)
         dgamma = dgamma_part.sum(1)
         del Tz
         del dP
@@ -967,21 +949,21 @@ class _IpaAttnTCFn(Function):
         kt[:, :, PQ3] = 1.0
         kt_hi, kt_lo = _planes_rows(kt.reshape(F_ * H_ * 32, N_))                                   # [F*H*32, n8]
         g1 = new(F_ * H_ * N_, 32)
-        _check(lib().dfold_gemm_bf16x3_batched(
-            _ptr(ds_hi), _ptr(ds_lo), F_ * H_, N_, N_, ds_hi.shape[1], F_ * H_, F_ * H_, 1, 0, N_,
-            _ptr(kt_hi), _ptr(kt_lo), F_ * H_, 32, N_, kt_hi.shape[1], 0, 0, 1, 32,
-            _ptr(g1), 32, F_ * H_ * N_, 1, 0, 1.0, _stream()), "dfold_gemm_bf16x3_batched")
+        launch("dfold_gemm_bf16x3_batched",
+               ds_hi, ds_lo, F_ * H_, N_, N_, ds_hi.shape[1], F_ * H_, F_ * H_, 1, 0, N_,
+               kt_hi, kt_lo, F_ * H_, 32, N_, kt_hi.shape[1], 0, 0, 1, 32,
+               g1, 32, F_ * H_ * N_, 1, 0, 1.0)
         qn = torch.zeros((F_, H_, N_, 32), dtype=torch.float32, device=dev)
         qh = q_pts.reshape(F_, N_, H_, PQ3).permute(0, 2, 1, 3)                                     # [F,H,N,24]
         qn[..., :PQ3] = qh
         qn[..., PQ3] = 1.0
         qn_hi, qn_lo = _planes_rows(qn.reshape(F_ * H_ * N_, 32))
         g2 = new(F_ * H_, N_, 32)
-        _check(lib().dfold_gemm_wgrad_bf16x3_batched(
-            _ptr(ds_hi), _ptr(ds_lo), N_, N_, F_ * H_, ds_hi.shape[1], N_ * ds_hi.shape[1],
-            _ptr(qn_hi), _ptr(qn_lo), 32, N_, F_ * H_, qn_hi.shape[1], N_ * qn_hi.shape[1],
-            32, 1, N_, F_ * H_, 0, 1, 0, 1, 0,
-            _ptr(g2), 32, N_ * 32, 1.0, _stream()), "dfold_gemm_wgrad_bf16x3_batched")
+        launch("dfold_gemm_wgrad_bf16x3_batched",
+               ds_hi, ds_lo, N_, N_, F_ * H_, ds_hi.shape[1], N_ * ds_hi.shape[1],
+               qn_hi, qn_lo, 32, N_, F_ * H_, qn_hi.shape[1], N_ * qn_hi.shape[1],
+               32, 1, N_, F_ * H_, 0, 1, 0, 1, 0,
+               g2, 32, N_ * 32, 1.0)
         g1 = g1.reshape(F_, H_, N_, 32)
         gam = gamma.reshape(1, H_, 1, 1)
         dq = -gam * (qh * g1[..., PQ3:PQ3 + 1] - g1[..., :PQ3])
@@ -990,26 +972,26 @@ class _IpaAttnTCFn(Function):
         dkv_pts.reshape(F_, N_, H_, W)[..., :PQ3] = dk.permute(0, 2, 1, 3)
         # ---- dV[j,h,c] = sum_{f,i} P[f,h,i,j] dO[f,i,h,c]   (MN-major, K over all frames) ----
         dkv = torch.zeros_like(kv)
-        _check(lib().dfold_gemm_wgrad_bf16x3_batched(
-            _ptr(p_hi), _ptr(p_lo), N_, N_, F_ * H_, n8, N_ * n8,
-            _ptr(dc_hi), _ptr(dc_lo), D, N_, F_, dc_hi.shape[1], N_ * dc_hi.shape[1],
-            C_, F_, N_, H_, H_, 1, 1, 0, C_,
-            _ptr(dkv, C_), H_ * 2 * C_, 2 * C_, 1.0, _stream()), "dfold_gemm_wgrad_bf16x3_batched")
+        launch("dfold_gemm_wgrad_bf16x3_batched",
+               p_hi, p_lo, N_, N_, F_ * H_, n8, N_ * n8,
+               dc_hi, dc_lo, D, N_, F_, dc_hi.shape[1], N_ * dc_hi.shape[1],
+               C_, F_, N_, H_, H_, 1, 1, 0, C_,
+               _ptr(dkv, C_), H_ * 2 * C_, 2 * C_, 1.0)
         # ---- dV_pts[f,j,h,e] = sum_i P[f,h,i,j] d_og[f,i,h,e] ----
         tmp = new(F_ * H_, N_, PV3)
-        _check(lib().dfold_gemm_wgrad_bf16x3_batched(
-            _ptr(p_hi), _ptr(p_lo), N_, N_, F_ * H_, n8, N_ * n8,
-            _ptr(dg_hi), _ptr(dg_lo), PV3, N_, F_ * H_, dg_hi.shape[1], N_ * dg_hi.shape[1],
-            PV3, 1, N_, F_ * H_, 0, 1, 0, 1, 0,
-            _ptr(tmp), PV3, N_ * PV3, 1.0, _stream()), "dfold_gemm_wgrad_bf16x3_batched")
+        launch("dfold_gemm_wgrad_bf16x3_batched",
+               p_hi, p_lo, N_, N_, F_ * H_, n8, N_ * n8,
+               dg_hi, dg_lo, PV3, N_, F_ * H_, dg_hi.shape[1], N_ * dg_hi.shape[1],
+               PV3, 1, N_, F_ * H_, 0, 1, 0, 1, 0,
+               tmp, PV3, N_ * PV3, 1.0)
         dkv_pts.reshape(F_, N_, H_, W)[..., PQ3:] = tmp.reshape(F_, H_, N_, PV3).permute(0, 2, 1, 3)
         # ---- dZ[i,j,c] = sum_{f,h} P[f,h,i,j] dOpair[f,i,h,c] ----
         dpair = new(1, N_, N_, Cp)
-        _check(lib().dfold_gemm_wgrad_bf16x3_batched(
-            _ptr(p_hi), _ptr(p_lo), N_, F_ * H_, N_, N_ * n8, n8,
-            _ptr(do_hi), _ptr(do_lo), Cp, F_ * H_, N_, do_hi.shape[1], F_ * H_ * do_hi.shape[1],
-            Cp, 1, F_ * H_, N_, 0, 1, 0, 1, 0,
-            _ptr(dpair), Cp, N_ * Cp, 1.0, _stream()), "dfold_gemm_wgrad_bf16x3_batched")
+        launch("dfold_gemm_wgrad_bf16x3_batched",
+               p_hi, p_lo, N_, F_ * H_, N_, N_ * n8, n8,
+               do_hi, do_lo, Cp, F_ * H_, N_, do_hi.shape[1], F_ * H_ * do_hi.shape[1],
+               Cp, 1, F_ * H_, N_, 0, 1, 0, 1, 0,
+               dpair, Cp, N_ * Cp, 1.0)
         dlogit0 = dS.sum(0, keepdim=True) if logit0.shape[0] == 1 else dS
         return dlogit0, dkv, dq_pts, dkv_pts, dpair, dquat, dtrans, None, dgamma, None, None, None, None, None
 
@@ -1054,9 +1036,8 @@ class _ScoreFn(Function):
         if x_pred is not None:
             trs = torch.empty(x_pred.shape[:-1] + (3,), dtype=torch.float64 if trans_f64 else torch.float32, device=q_pred.device)
         max_s, min_s, min_b, max_b, r3, ipa, L = consts
-        _check(lib().dfold_score_fwd(_ptr(q_pred), _ptr(q_t), _ptr(x_pred), _ptr(x_t), _ptr(t64), _ptr(grid), grid.numel(),
-                                     max_s, min_s, min_b, max_b, r3, ipa, _ptr(mask), L, n, _ptr(rot), _ptr(trs), int(trans_f64),
-                                     _stream()), "dfold_score_fwd")
+        launch("dfold_score_fwd", q_pred, q_t, x_pred, x_t, t64, grid, grid.numel(),
+               max_s, min_s, min_b, max_b, r3, ipa, mask, L, n, rot, trs, int(trans_f64))
         ctx.save_for_backward(q_pred, q_t, x_pred, x_t, t64, grid, mask)
         ctx.meta = (consts, trans_f64)
         return rot, trs
@@ -1072,9 +1053,8 @@ class _ScoreFn(Function):
         d_trs = d_trs.to(torch.float64 if trans_f64 else torch.float32).contiguous() if d_trs is not None else None
         dq = torch.empty_like(q_pred)
         dx = torch.empty_like(x_pred) if x_pred is not None else None
-        _check(lib().dfold_score_bwd(_ptr(q_pred), _ptr(q_t), _ptr(x_pred), _ptr(x_t), _ptr(t64), _ptr(grid), grid.numel(),
-                                     max_s, min_s, min_b, max_b, r3, ipa, _ptr(mask), L, n, _ptr(d_rot), _ptr(d_trs), int(trans_f64),
-                                     _ptr(dq), _ptr(dx), _stream()), "dfold_score_bwd")
+        launch("dfold_score_bwd", q_pred, q_t, x_pred, x_t, t64, grid, grid.numel(),
+               max_s, min_s, min_b, max_b, r3, ipa, mask, L, n, d_rot, d_trs, int(trans_f64), dq, dx)
         return dq, None, dx, None, None, None, None, None, None
 
 
@@ -1105,10 +1085,9 @@ class _FramesToAtomsFn(Function):
         a14 = torch.empty(lead + (14, 3), dtype=torch.float32, device=dev)
         a37 = torch.empty(lead + (37, 3), dtype=torch.float32, device=dev)
         fr = torch.empty(lead + (8, 4, 4), dtype=torch.float32, device=dev) if want_frames else None
-        _check(lib().dfold_frames_to_atoms_fwd(_ptr(rotc), int(rot_is_matrix), _ptr(transc), _ptr(alphac), _ptr(aac),
-                                               *[_ptr(tables[k]) for k in ("default_frames", "atom14_group", "atom14_mask",
-                                                                           "atom14_pos", "atom37_to_atom14", "atom37_mask")],
-                                               _ptr(fr), _ptr(a14), _ptr(a37), n, _stream()), "dfold_frames_to_atoms_fwd")
+        launch("dfold_frames_to_atoms_fwd", rotc, int(rot_is_matrix), transc, alphac, aac,
+               *[tables[k] for k in ("default_frames", "atom14_group", "atom14_mask", "atom14_pos", "atom37_to_atom14", "atom37_mask")],
+               fr, a14, a37, n)
         ctx.save_for_backward(rotc, transc, alphac, aac)
         ctx.eager = eager
         ctx.want_frames = want_frames
@@ -1145,7 +1124,7 @@ class _QuatMulFn(Function):
         out = torch.empty(shp + (4,), dtype=torch.float32, device=a.device)
         n = out.numel() // 4
         if n:
-            _check(lib().dfold_quat_mul_fwd(_ptr(ac), _ptr(bc), _ptr(out), n, int(b_is_vec), _stream()), "dfold_quat_mul_fwd")
+            launch("dfold_quat_mul_fwd", ac, bc, out, n, int(b_is_vec))
         ctx.save_for_backward(ac, bc)
         ctx.meta = (a.shape, b.shape, b_is_vec)
         return out
@@ -1159,7 +1138,7 @@ class _QuatMulFn(Function):
         da, db = torch.empty_like(ac), torch.empty_like(bc)
         n = ac.numel() // 4
         if n:
-            _check(lib().dfold_quat_mul_bwd(_ptr(ac), _ptr(bc), _ptr(g), _ptr(da), _ptr(db), n, int(b_is_vec), _stream()), "dfold_quat_mul_bwd")
+            launch("dfold_quat_mul_bwd", ac, bc, g, da, db, n, int(b_is_vec))
         return da.sum_to_size(ashape) if da.shape != ashape else da, db.sum_to_size(bshape) if db.shape != bshape else db, None
 
 
@@ -1212,8 +1191,7 @@ class _RotComposeFn(Function):
         Ro = torch.empty(out_lead + (3, 3), dtype=torch.float32, device=dev) if Rbc is not None else None
         to = torch.empty(out_lead + (3,), dtype=torch.float32, device=dev) if tbc is not None else None
         if na:
-            _check(lib().dfold_rot_compose_fwd(_ptr(Rac), _ptr(tac), _ptr(Rbc), _ptr(tbc), _ptr(Ro), _ptr(to), na, rep, int(inverse),
-                                               _stream()), "dfold_rot_compose_fwd")
+            launch("dfold_rot_compose_fwd", Rac, tac, Rbc, tbc, Ro, to, na, rep, int(inverse))
         ctx.save_for_backward(Rac, tac, Rbc, tbc)
         ctx.meta = (tuple(Ra.shape), tuple(ta.shape) if ta is not None else None, tuple(Rb.shape) if Rb is not None else None,
                     tuple(tb.shape) if tb is not None else None, rep, inverse, na)
@@ -1232,8 +1210,7 @@ class _RotComposeFn(Function):
         dRb = torch.empty_like(Rbc) if Rbc is not None else None
         dtb = torch.empty_like(tbc) if tbc is not None else None
         if na:
-            _check(lib().dfold_rot_compose_bwd(_ptr(Rac), _ptr(tac), _ptr(Rbc), _ptr(tbc), _ptr(dRo), _ptr(dto), _ptr(dRa), _ptr(dta),
-                                               _ptr(dRb), _ptr(dtb), na, rep, int(inverse), _stream()), "dfold_rot_compose_bwd")
+            launch("dfold_rot_compose_bwd", Rac, tac, Rbc, tbc, dRo, dto, dRa, dta, dRb, dtb, na, rep, int(inverse))
 
         def fit(g, shape):
             if g is None or shape is None:
@@ -1261,10 +1238,9 @@ def reverse_step(q_t, x_t, rot_score, trans_score, z_rot, z_trans, mask, *, g_ro
         mk = _f32c(mask) if mask is not None else None
         F_, N_ = q_t.shape[0], q_t.shape[1]
         q_out, x_out = torch.empty_like(q_t), torch.empty_like(x_t)
-        _check(lib().dfold_reverse_step(_ptr(q_t), _ptr(x_t), _ptr(rs), _ptr(ts), int(ts.dtype == torch.float64), _ptr(z_rot), _ptr(z_trans),
-                                        _ptr(mk), float(g_rot), float(g_trans), float(b_t), float(dt), float(noise_scale), float(r3_scale),
-                                        int(center), int(diffuse_rot), int(diffuse_trans), _ptr(q_out), _ptr(x_out), F_, N_, _stream()),
-               "dfold_reverse_step")
+        launch("dfold_reverse_step", q_t, x_t, rs, ts, int(ts.dtype == torch.float64), z_rot, z_trans,
+               mk, float(g_rot), float(g_trans), float(b_t), float(dt), float(noise_scale), float(r3_scale),
+               int(center), int(diffuse_rot), int(diffuse_trans), q_out, x_out, F_, N_)
     return q_out, x_out
 
 
@@ -1277,7 +1253,7 @@ def igso3_tables(sigma_grid, num_omega: int, L: int = 1000):
         G = g.numel()
         cdf = torch.empty(G, num_omega, dtype=torch.float64, device=g.device)
         scaling = torch.empty(G, dtype=torch.float64, device=g.device)
-        _check(lib().dfold_igso3_tables(_ptr(g), G, int(num_omega), int(L), _ptr(cdf), _ptr(scaling), _stream()), "dfold_igso3_tables")
+        launch("dfold_igso3_tables", g, G, int(num_omega), int(L), cdf, scaling)
     return cdf, scaling
 
 
@@ -1302,11 +1278,9 @@ def forward_marginal(rigids_0, z_axis, u, z_trans, mask, t64, grid, cdf, score_s
             ts = torch.empty(n, 3, dtype=torch.float64, device=dev)
             sc = torch.empty(2, dtype=torch.float64, device=dev)
             rsc, tsc = sc[0], sc[1]
-        _check(lib().dfold_forward_marginal(_ptr(r0), _ptr(za), _ptr(uu), _ptr(zt), _ptr(mk), _ptr(t64), _ptr(grid), _ptr(cdf),
-                                            _ptr(score_scaling), grid.numel(), cdf.shape[1], int(L), float(max_sigma),
-                                            float(min_sigma), float(min_b), float(max_b), float(r3_scale), int(diffuse_rot),
-                                            int(diffuse_trans), int(ref_mode), _ptr(rig), _ptr(rs), _ptr(ts), _ptr(rsc), _ptr(tsc),
-                                            n, _stream()), "dfold_forward_marginal")
+        launch("dfold_forward_marginal", r0, za, uu, zt, mk, t64, grid, cdf, score_scaling, grid.numel(), cdf.shape[1], int(L),
+               float(max_sigma), float(min_sigma), float(min_b), float(max_b), float(r3_scale), int(diffuse_rot),
+               int(diffuse_trans), int(ref_mode), rig, rs, ts, rsc, tsc, n)
     return rig, rs, ts, rsc, tsc
 
 
@@ -1338,5 +1312,4 @@ def rollout_advance(rigid_pred, atom37, rigids_0, rigid_traj, atom_traj, step):
                          f"{tuple(rigid_traj.shape)} and {tuple(atom_traj.shape)}")
     with torch.cuda.device(rigids_0.device):
         rp, a37 = rigid_pred.detach().contiguous(), atom37.detach().contiguous()
-        _check(lib().dfold_rollout_advance(_ptr(rp), _ptr(a37), _ptr(rigids_0), _ptr(rigid_traj), _ptr(atom_traj), _ptr(step),
-                                           nf, N, A, L, _stream()), "dfold_rollout_advance")
+        launch("dfold_rollout_advance", rp, a37, rigids_0, rigid_traj, atom_traj, step, nf, N, A, L)

@@ -31,10 +31,8 @@ class _LossFn(Function):
         out = torch.empty(8, dtype=torch.float64, device=dev)
         d_ang, d_rs, d_x = torch.empty_like(ang), torch.empty_like(rs), torch.empty_like(x)
         w_tor, w_rot, w_trans, t_thr, rot_on, separate = consts
-        K._check(K.lib().dfold_loss_fwd(K._ptr(ang), K._ptr(a_gt), K._ptr(a_alt), K._ptr(a_mask), K._ptr(rs), K._ptr(gt_rot),
-                                        K._ptr(x), K._ptr(x0), K._ptr(res_mask), K._ptr(fixed_mask), K._ptr(t), K._ptr(scaling),
-                                        nf, N, float(w_tor), float(w_rot), float(w_trans), float(t_thr), int(rot_on), int(separate),
-                                        K._ptr(out), K._ptr(d_ang), K._ptr(d_rs), K._ptr(d_x), K._stream()), "dfold_loss_fwd")
+        K.launch("dfold_loss_fwd", ang, a_gt, a_alt, a_mask, rs, gt_rot, x, x0, res_mask, fixed_mask, t, scaling,
+                 nf, N, float(w_tor), float(w_rot), float(w_trans), float(t_thr), int(rot_on), int(separate), out, d_ang, d_rs, d_x)
         ctx.save_for_backward(d_ang, d_rs, d_x)
         ctx.meta = (angles.shape, angles.dtype, rot_score.shape, rot_score.dtype, rigids.shape, rigids.dtype)
         return out

@@ -55,8 +55,7 @@ def rot_trans_error(pred_rigids: torch.Tensor, gt_rigids: torch.Tensor, ref_fram
         p, p64 = _src(pred_rigids)
         g, g64 = _src(gt_rigids)
         out = _f64(4, nf, device=dev)
-        K._check(K.lib().dfold_rot_trans_error(K._ptr(p), p64, K._ptr(g), g64, nf, N, rf, K._ptr(out), K._stream()),
-                 "dfold_rot_trans_error")
+        K.launch("dfold_rot_trans_error", p, p64, g, g64, nf, N, rf, out)
     return out[0], out[1], out[2], out[3]
 
 
@@ -77,8 +76,7 @@ def atom_errors(atom37_pred: torch.Tensor, atom37_gt: torch.Tensor, atom37_mask:
         g, g64 = _src(atom37_gt)
         m, m64 = _src(atom37_mask)
         out = _f64(6, nf, device=dev)
-        K._check(K.lib().dfold_atom_errors(K._ptr(p), p64, K._ptr(g), g64, K._ptr(m), m64, nf, N, A, int(bool(drop_last_atom)),
-                                           K._ptr(out), K._stream()), "dfold_atom_errors")
+        K.launch("dfold_atom_errors", p, p64, g, g64, m, m64, nf, N, A, int(bool(drop_last_atom)), out)
     return {"mae": out[0], "mse": out[1], "rmsd_all": out[2], "rmsd_ca": out[3]}
 
 
@@ -88,10 +86,8 @@ def _superimpose(ref, ref64, x, x64, offset, sstride, pstride, mask, m64, moff, 
     coords = _f64(B, P, 3, device=dev) if with_coords else None
     rot = _f64(B, 3, 3, device=dev) if with_transform else None
     trans = _f64(B, 3, device=dev) if with_transform else None
-    K._check(K.lib().dfold_superimpose(K._ptr(ref, offset), ref64, K._ptr(x, offset), x64, sstride, pstride,
-                                       K._ptr(mask, moff) if mask is not None else None, m64, msstride, mpstride, mode, B, P,
-                                       K._ptr(rmsd), K._ptr(rot), K._ptr(trans), K._ptr(coords), K._stream()),
-             "dfold_superimpose")
+    K.launch("dfold_superimpose", K._ptr(ref, offset), ref64, K._ptr(x, offset), x64, sstride, pstride,
+             K._ptr(mask, moff), m64, msstride, mpstride, mode, B, P, rmsd, rot, trans, coords)
     return coords, rmsd, rot, trans
 
 
@@ -133,9 +129,8 @@ def _drmsd(s1, a64, s2, b64, offset, sstride, pstride, mask, m64, moff, msstride
         raise ValueError(f"drmsd: {B} structure pairs exceed 65535")
     partial = _f64(B * T * T, device=dev)
     out = _f64(B, device=dev)
-    K._check(K.lib().dfold_drmsd(K._ptr(s1, offset), a64, K._ptr(s2, offset), b64, sstride, pstride,
-                                 K._ptr(mask, moff) if mask is not None else None, m64, msstride, mpstride, int(premul), B, N,
-                                 K._ptr(partial), K._ptr(out), K._stream()), "dfold_drmsd")
+    K.launch("dfold_drmsd", K._ptr(s1, offset), a64, K._ptr(s2, offset), b64, sstride, pstride,
+             K._ptr(mask, moff), m64, msstride, mpstride, int(premul), B, N, partial, out)
     return out
 
 

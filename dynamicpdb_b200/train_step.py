@@ -155,11 +155,9 @@ class TrainStep:
         self.loss.copy_(loss.detach().float())
 
     def _adam(self, a: int, b: int, tick: bool):
-        K = _kernels
-        K._check(K.lib().dfold_adam_amsgrad(K._ptr(self.flat_param, a), K._ptr(self.flat_grad, a), K._ptr(self.exp_avg, a),
-                                            K._ptr(self.exp_avg_sq, a), K._ptr(self.max_exp_avg_sq, a), b - a,
-                                            K._ptr(self.step_count), 1 if tick else 0, self.lr, 0.9, 0.999, 1e-8,
-                                            1.0 / self.world, K._stream()), "dfold_adam_amsgrad")
+        _kernels.launch("dfold_adam_amsgrad", self.flat_param[a:b], self.flat_grad[a:b], self.exp_avg[a:b], self.exp_avg_sq[a:b],
+                        self.max_exp_avg_sq[a:b], b - a, self.step_count, 1 if tick else 0, self.lr, 0.9, 0.999, 1e-8,
+                        1.0 / self.world)
 
     def optimizer_step(self):
         if self.opt is not None:

@@ -208,10 +208,9 @@ def test_two_launches_same_bits_and_nothing_else_written():
         rs = torch.full((n * 3 + 2 * pad,), float("nan"), dtype=torch.float64, device=DEV)
         ts = torch.full_like(rs, float("nan"))
         scal = torch.full((2 + 2 * pad,), float("nan"), dtype=torch.float64, device=DEV)
-        K._check(K.lib().dfold_forward_marginal(K._ptr(rig7), K._ptr(za), K._ptr(u), K._ptr(zt), None, K._ptr(t64), K._ptr(grid),
-                                                K._ptr(cdf), K._ptr(sc), grid.numel(), cdf.shape[1], 1000, 1.5, 0.1, 0.1, 20.0, 0.1,
-                                                1, 1, 0, K._ptr(rig, pad), K._ptr(rs, pad), K._ptr(ts, pad), K._ptr(scal, pad),
-                                                K._ptr(scal, pad + 1), n, K._stream()), "dfold_forward_marginal")
+        K.launch("dfold_forward_marginal", rig7, za, u, zt, None, t64, grid, cdf, sc, grid.numel(), cdf.shape[1], 1000, 1.5, 0.1,
+                 0.1, 20.0, 0.1, 1, 1, 0, K._ptr(rig, pad), K._ptr(rs, pad), K._ptr(ts, pad), K._ptr(scal, pad),
+                 K._ptr(scal, pad + 1), n)
         for buf, m in ((rig, n * 7), (rs, n * 3), (ts, n * 3), (scal, 2)):
             assert bool(torch.isnan(buf[:pad]).all()) and bool(torch.isnan(buf[pad + m:]).all())
             assert bool(torch.isfinite(buf[pad:pad + m]).all())

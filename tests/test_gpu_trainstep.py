@@ -101,8 +101,7 @@ def test_fused_adam_matches_torch_adam_amsgrad():
         grad[:100] = 0
         ref.grad = grad.clone()
         opt.step()
-        K._check(K.lib().dfold_adam_amsgrad(K._ptr(p), K._ptr(grad), K._ptr(m), K._ptr(v), K._ptr(vm), n, K._ptr(step), 1,
-                                            1e-3, 0.9, 0.999, 1e-8, 1.0, K._stream()), "dfold_adam_amsgrad")
+        K.launch("dfold_adam_amsgrad", p, grad, m, v, vm, n, step, 1, 1e-3, 0.9, 0.999, 1e-8, 1.0)
         assert (p - ref.detach()).abs().max().item() < 2e-6 * max(1.0, ref.abs().max().item()), it
     assert torch.equal(p[:100], p0[:100]) and float(step) == 6.0
 
