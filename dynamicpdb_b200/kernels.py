@@ -998,18 +998,19 @@ class _IpaAttnTCFn(Function):
 
 def _tc_path_ok(logit0, kv, q_pts, pair, Pq, Pv) -> bool:
     """The tensor-core decomposition is built for the DFOLDv2 preset-A head geometry (H 8, Pq 8, Pv 12, Cp 32: the fused
-    forward csrc/ipa_fused.cu and the dS kernel csrc/ipa_v2.cu) and needs frame-shared q/k/v and pair tensors, a head
-    width that is a whole number of 64-wide K blocks and rows that fit in shared memory."""
+    forward csrc/ipa_fused.cu and the dS kernel csrc/ipa_v2.cu) and needs frame-shared logit0, q/k/v and pair tensors (the
+    fused forward reads logit0 as one [H,N,N] with no frame stride), a head width that is a whole number of 64-wide K
+    blocks and rows that fit in shared memory."""
     C_ = kv.shape[-1] // 2
     N_, H_ = q_pts.shape[1], q_pts.shape[2]
-    return (H_ == 8 and Pq == 8 and Pv == 12 and pair.shape[-1] == 32
+    return (H_ == 8 and Pq == 8 and Pv == 12 and pair.shape[-1] == 32 and logit0.shape[0] == 1
             and kv.shape[0] == 1 and pair.shape[0] == 1 and C_ % 64 == 0 and N_ <= 1280 and N_ % 8 == 0)
 
 
 def ipa_attention(logit0, kv, q_pts, kv_pts, pair, quat, trans, mask, gamma, *, Pq, Pv, dfold, inf, eps):
     """IPA core -> concat buffer [F,N,D] in the reference's feature order.
 
-    The preset-A head geometry with frame-shared q/k/v, C % 64 == 0 and N <= 1280 (DFOLDv2) runs the tensor-core
+    The preset-A head geometry with frame-shared logit0, q/k/v and pair, C % 64 == 0 and N <= 1280 (DFOLDv2) runs the tensor-core
     decomposition (csrc/ipa_fused.cu, csrc/ipa_v2.cu); every other shape runs the single fused CUDA-core kernel
     (csrc/ipa_attn.cu).  Both are this library's kernels."""
     if _tc_path_ok(logit0, kv, q_pts, pair, Pq, Pv):

@@ -203,12 +203,14 @@ def test_qk_logits(Fs, Fz):
     check("qk_logits", [R(Fs, N, H, C), R(Fs, N, H, 2 * C), b.detach().requires_grad_(True), 0.25, 0.577], 2e-5)
 
 
-def _ipa_inputs(F, N, H, C, Pq, Pv, Cp, Fs, Fz, masked):
+def _ipa_inputs(F, N, H, C, Pq, Pv, Cp, Fs, Fz, masked, Fl=None):
+    """Fl: frames of logit0, max(Fs, Fz) (what layers.ipa_forward builds) unless given."""
     mask = torch.ones(F, N)
     if masked:
         mask[:, -3:] = 0
         mask[0, 1] = 0
-    return [R(max(Fs, Fz), H, N, N), R(Fs, N, H, 2 * C), R(F, N, H, Pq, 3, scale=4.0), R(F, N, H, Pq + Pv, 3, scale=4.0),
+    Fl = max(Fs, Fz) if Fl is None else Fl
+    return [R(Fl, H, N, N), R(Fs, N, H, 2 * C), R(F, N, H, Pq, 3, scale=4.0), R(F, N, H, Pq + Pv, 3, scale=4.0),
             R(Fz, N, N, Cp), unit(F, N, 4), R(F, N, 3, scale=8.0), mask, (torch.rand(H) * 0.2 + 0.05).requires_grad_(True)]
 
 
@@ -242,6 +244,17 @@ def test_ipa_attention(F, N, H, C, Pq, Pv, Cp, Fs, Fz, dfold, masked):
     # atomic accumulation order, and the split-bf16 value-point term of dS (2^-17 per product) by up to ~7e-4
     check("ipa_attention", inputs, 2e-4, post=post, grad_tol={7: 1.5e-3}, ref_device=dev, Pq=Pq, Pv=Pv, dfold=dfold, inf=1e5,
           eps=1e-8)
+
+
+@pytest.mark.parametrize("masked", [False, True])
+def test_ipa_attention_per_frame_logit0(masked):
+    """Per-frame logit0 [F,H,N,N] with frame-shared kv and pair at the preset-A head geometry: the header allows it, and
+    the fused forward (which reads one [H,N,N] logit0 with no frame stride) must not take it.  Kept apart from
+    test_ipa_attention because a logit0-frames column there would rename every existing case."""
+    F, N, H, C, Pq, Pv, Cp = 3, 40, 8, 256, 8, 12, 32
+    inputs = _ipa_inputs(F, N, H, C, Pq, Pv, Cp, 1, 1, masked, Fl=F)
+    post = lambda out, *a: out * a[7][:, :, None]
+    check("ipa_attention", inputs, 2e-4, post=post, grad_tol={7: 1.5e-3}, Pq=Pq, Pv=Pv, dfold=True, inf=1e5, eps=1e-8)
 
 
 @pytest.mark.parametrize("F,N,Ci,Co,crop", [(7, 24, 64, 128, 2), (17, 40, 160, 80, 2), (5, 130, 128, 64, 4), (8, 256, 1280, 640, 3)])
