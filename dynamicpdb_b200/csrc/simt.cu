@@ -602,17 +602,21 @@ namespace dfold {
 namespace {
 __global__ void adam_tick_kernel(float* step) { *step += 1.f; }
 
+// kClip: the gradient is ((g * gscale) * *coef), the order of DDP's mean followed by clip_grad_norm_'s mul_(coef).
+template <bool kClip>
 __global__ void __launch_bounds__(256) adam_amsgrad_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                            float* __restrict__ v, float* __restrict__ vmax, long n4,
                                                            const float* __restrict__ step, float lr, float b1, float b2, float eps,
-                                                           float gscale) {
+                                                           float gscale, const float* __restrict__ coef) {
     const float t = *step;
     const float bc1 = 1.f - powf(b1, t), bc2 = 1.f - powf(b2, t);
     const float step_size = lr / bc1, inv_bc2_sqrt = 1.f / sqrtf(bc2);
+    const float c = kClip ? *coef : 1.f;
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
         float4 P = reinterpret_cast<float4*>(p)[i];
         float4 G = reinterpret_cast<const float4*>(g)[i];
         G.x *= gscale; G.y *= gscale; G.z *= gscale; G.w *= gscale;      // 1 / world_size of the data-parallel mean
+        if (kClip) { G.x *= c; G.y *= c; G.z *= c; G.w *= c; }
         float4 M = reinterpret_cast<float4*>(m)[i], V = reinterpret_cast<float4*>(v)[i], X = reinterpret_cast<float4*>(vmax)[i];
         float* pp = &P.x; const float* gg = &G.x; float* mm = &M.x; float* vv = &V.x; float* xx = &X.x;
 #pragma unroll
@@ -628,21 +632,110 @@ __global__ void __launch_bounds__(256) adam_amsgrad_kernel(float* __restrict__ p
         reinterpret_cast<float4*>(vmax)[i] = X;
     }
 }
+
+// ---------------------------------------------------------------------------------------------------
+// Global L2 norm of the flat gradient and the clipping coefficient of torch.nn.utils.clip_grad_norm_ (norm_type 2), the
+// optimizer-side option of the reference trainer (train_DFOLD_dynamics.py:665).  The order of the sum depends on n only, not
+// on the device, so every run and every data-parallel rank (all reduce the same all-reduced buffer) gets the same bits:
+// CTA b of grad_norm_blocks(n / 4) has thread t add, in turn, the squares of float4s b 256 + t, + 256 blocks, ... in fp64
+// (the square of an fp32 value is exact there); then the 32 lanes by xor butterfly and the 8 warp sums in warp order.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kNormThreads = 256, kNormMaxBlocks = 1024;
+
+static inline int grad_norm_blocks(long n4) {
+    return (int)(cdiv(n4, kNormThreads) < kNormMaxBlocks ? cdiv(n4, kNormThreads) : kNormMaxBlocks);
+}
+
+// sum over the CTA's 256 threads (valid in thread 0)
+__device__ __forceinline__ double norm_block_sum(double s) {
+    __shared__ double red[kNormThreads / 32];
+    s = warp_sum_d(s);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    double t = 0.0;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < kNormThreads / 32; ++w) t += red[w];
+    return t;
+}
+
+__global__ void __launch_bounds__(kNormThreads) grad_sqnorm_partial_kernel(const float* __restrict__ g, long n4,
+                                                                           double* __restrict__ partial) {
+    double s = 0.0;
+    for (long i = (long)blockIdx.x * kNormThreads + threadIdx.x; i < n4; i += (long)gridDim.x * kNormThreads) {
+        const float4 G = reinterpret_cast<const float4*>(g)[i];
+        const double x = G.x, y = G.y, z = G.z, w = G.w;
+        s = fma(x, x, s); s = fma(y, y, s); s = fma(z, z, s); s = fma(w, w, s);
+    }
+    s = norm_block_sum(s);
+    if (threadIdx.x == 0) partial[blockIdx.x] = s;
+}
+
+// One CTA: thread t adds partials t, t + 256, ... in turn, then as above.  total = fp32(sqrt(sum) gscale), and the
+// coefficient in fp32 as torch evaluates max_norm / (total + 1e-6) (Tensor.__rtruediv__: reciprocal, then the product)
+// clamped to at most 1, where a NaN stays NaN as in torch.clamp.
+__global__ void __launch_bounds__(kNormThreads) grad_norm_finalize_kernel(const double* __restrict__ partial, int nblocks,
+                                                                          float gscale, float max_norm,
+                                                                          float* __restrict__ total, float* __restrict__ coef) {
+    double s = 0.0;
+    for (int i = threadIdx.x; i < nblocks; i += kNormThreads) s += partial[i];
+    s = norm_block_sum(s);
+    if (threadIdx.x == 0) {
+        const float tn = (float)(sqrt(s) * (double)gscale);
+        const float c = __fmul_rn(__frcp_rn(__fadd_rn(tn, 1e-6f)), max_norm);
+        *total = tn;
+        *coef = (c > 1.f) ? 1.f : c;
+    }
+}
 }  // namespace
+
+static int adam_launch(bool clip, float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq,
+                       long n, float* step, int tick, float lr, float beta1, float beta2, float eps, float grad_scale,
+                       const float* coef, cudaStream_t st) {
+    if (tick) adam_tick_kernel<<<1, 1, 0, st>>>(step);            // chunked callers advance the step once per optimizer step
+    const long n4 = n / 4;
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
+        sms = 132;
+    const long cap = 16L * sms;                                     // 16 CTAs of 256 threads per SM, grid-stride beyond
+    const int blocks = (int)(cdiv(n4, 256) < cap ? cdiv(n4, 256) : cap);
+    if (clip)
+        adam_amsgrad_kernel<true><<<blocks, 256, 0, st>>>(param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n4, step, lr, beta1,
+                                                          beta2, eps, grad_scale, coef);
+    else
+        adam_amsgrad_kernel<false><<<blocks, 256, 0, st>>>(param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n4, step, lr, beta1,
+                                                           beta2, eps, grad_scale, nullptr);
+    return check_launch("adam_amsgrad_kernel");
+}
 }  // namespace dfold
 
 // n must be a multiple of 4 and the buffers 16-byte aligned (train_step.py pads its flat buffers).
 extern "C" int dfold_adam_amsgrad(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, long n,
                                   float* step, int tick, float lr, float beta1, float beta2, float eps, float grad_scale, void* stream) {
     DFOLD_REQUIRE(n > 0 && n % 4 == 0, "dfold_adam_amsgrad: n must be a positive multiple of 4");
+    return dfold::adam_launch(false, param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n, step, tick, lr, beta1, beta2, eps,
+                              grad_scale, nullptr, dfold::as_stream(stream));
+}
+
+extern "C" int dfold_adam_amsgrad_clip(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq,
+                                       long n, float* step, int tick, float lr, float beta1, float beta2, float eps, float grad_scale,
+                                       const float* coef, void* stream) {
+    DFOLD_REQUIRE(n > 0 && n % 4 == 0, "dfold_adam_amsgrad_clip: n must be a positive multiple of 4");
+    DFOLD_REQUIRE(coef != nullptr, "dfold_adam_amsgrad_clip: null coefficient");
+    return dfold::adam_launch(true, param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n, step, tick, lr, beta1, beta2, eps,
+                              grad_scale, coef, dfold::as_stream(stream));
+}
+
+// partial: workspace of at least 1024 doubles.
+extern "C" int dfold_grad_norm(const float* grad, long n, float grad_scale, float max_norm, double* partial, float* total,
+                               float* coef, void* stream) {
+    DFOLD_REQUIRE(n > 0 && n % 4 == 0, "dfold_grad_norm: n must be a positive multiple of 4");
+    DFOLD_REQUIRE(max_norm > 0.f, "dfold_grad_norm: max_norm must be positive (inf reports the norm without clipping)");
+    DFOLD_REQUIRE(partial != nullptr && total != nullptr && coef != nullptr, "dfold_grad_norm: null workspace or output");
     cudaStream_t st = dfold::as_stream(stream);
-    if (tick) dfold::adam_tick_kernel<<<1, 1, 0, st>>>(step);      // chunked callers advance the step once per optimizer step
     const long n4 = n / 4;
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-        sms = 132;
-    const long cap = 16L * sms;                                     // 16 CTAs of 256 threads per SM, grid-stride beyond
-    const int blocks = (int)(dfold::cdiv(n4, 256) < cap ? dfold::cdiv(n4, 256) : cap);
-    dfold::adam_amsgrad_kernel<<<blocks, 256, 0, st>>>(param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n4, step, lr, beta1, beta2, eps, grad_scale);
-    return dfold::check_launch("adam_amsgrad_kernel");
+    const int blocks = dfold::grad_norm_blocks(n4);
+    dfold::grad_sqnorm_partial_kernel<<<blocks, dfold::kNormThreads, 0, st>>>(grad, n4, partial);
+    if (dfold::check_launch("grad_sqnorm_partial_kernel")) return 1;
+    dfold::grad_norm_finalize_kernel<<<1, dfold::kNormThreads, 0, st>>>(partial, blocks, grad_scale, max_norm, total, coef);
+    return dfold::check_launch("grad_norm_finalize_kernel");
 }

@@ -57,6 +57,8 @@ _SIGS = {
     "dfold_frames_to_atoms_fwd": "pippp" + "pppppp" + "ppp" + "lp",
     "dfold_reverse_step": "ppppi" + "ppp" + "dddddd" + "iii" + "pp" + "llp",
     "dfold_adam_amsgrad": "pppppl" + "pi" + "fffff" + "p",
+    "dfold_adam_amsgrad_clip": "pppppl" + "pi" + "fffff" + "pp",
+    "dfold_grad_norm": "plff" + "ppp" + "p",
     "dfold_featurize_window": "pppppp" + "ii" + "pppp" + "p",
     "dfold_loss_fwd": "pppppppppppp" + "ii" + "dddd" + "ii" + "pppp" + "p",
     "dfold_quat_mul_fwd": "ppplip",
@@ -98,7 +100,8 @@ def exported_symbols():
 
 
 # kernels launched per C-ABI call (bench.py reports the total as `gpu_launches`)
-_LAUNCHES_PER_CALL = {"dfold_global_layernorm_fwd": 3, "dfold_global_layernorm_bwd": 3, "dfold_ipa_attn_bwd": 4}
+_LAUNCHES_PER_CALL = {"dfold_global_layernorm_fwd": 3, "dfold_global_layernorm_bwd": 3, "dfold_ipa_attn_bwd": 4,
+                      "dfold_grad_norm": 2}
 LAUNCH_COUNT = 0
 # When True (set by train_step.TrainStep around its step), weight gradients of the convolution are accumulated by the kernel
 # straight into the parameter's existing .grad buffer and autograd receives None: the ConvNet is shared by the four blocks

@@ -13,10 +13,14 @@ comparable to the device time, so the step is:
 * ``torch.cuda.graph`` captures the whole step (the C-ABI kernels are plain stream launches; TMA descriptors are
   by-value kernel arguments), replays have no Python / launch overhead;
 * if capture is not possible the same step runs eagerly (``graph=False`` or on capture failure);
+* ``max_grad_norm`` clips the data-parallel mean gradient by its global norm inside the same graph, as
+  ``torch.nn.utils.clip_grad_norm_`` between ``loss.backward()`` and ``optimizer.step()`` would (the option the reference
+  trainer keeps commented out, train_DFOLD_dynamics.py:665); ``grad_norm`` holds the norm before clipping;
 * ``state_dict()`` / ``load_state_dict()`` save and resume the weights and the Adam(amsgrad) state in the reference
   trainer's checkpoint format, loading in place so the captured graph keeps running (checkpoint.py).
 """
 import copy
+import numbers
 import os
 import sys
 import time
@@ -32,7 +36,14 @@ from . import kernels as _kernels
 class TrainStep:
     def __init__(self, net: torch.nn.Module, loss_fn: Callable[[Dict[str, torch.Tensor]], torch.Tensor],
                  example_feats: Dict[str, torch.Tensor], *, lr: float = 1e-4, world_size: int = 1, graph: bool = True,
-                 warmup: int = 3):
+                 warmup: int = 3, max_grad_norm: Optional[float] = None):
+        self.max_grad_norm = _check_max_grad_norm(max_grad_norm)
+        self.fused_adam = os.environ.get("DFOLD_TORCH_ADAM", "0") != "1"
+        self.chunks = max(1, int(os.environ.get("DFOLD_ALLREDUCE_CHUNKS", "1")))
+        if self.max_grad_norm is not None and self.fused_adam and world_size > 1 and self.chunks > 1:
+            raise ValueError("max_grad_norm needs the whole all-reduced gradient before the first update, but "
+                             f"DFOLD_ALLREDUCE_CHUNKS={self.chunks} updates each piece as soon as it is reduced: "
+                             "unset it to clip")
         self.net, self.loss_fn, self.world = net, loss_fn, world_size
         self.params = [p for p in net.parameters() if p.requires_grad]
         self.layout = _ckpt.flat_layout(net)             # where each trained parameter sits in the flat buffers
@@ -42,9 +53,7 @@ class TrainStep:
         # Adam(amsgrad) as the reference trainer (train_DFOLD_dynamics.py:412).  Default: ONE fused kernel over flat
         # parameter / gradient / moment buffers (csrc/simt.cu adam_amsgrad_kernel, step counter on the device); with
         # DFOLD_TORCH_ADAM=1: torch.optim.Adam(capturable, foreach) on the same gradient views.
-        self.fused_adam = os.environ.get("DFOLD_TORCH_ADAM", "0") != "1"
         self.lr = lr
-        self.chunks = max(1, int(os.environ.get("DFOLD_ALLREDUCE_CHUNKS", "1")))
         if self.fused_adam:
             self.flat_param = torch.zeros(padded, dtype=torch.float32, device=dev)
         off = 0
@@ -67,6 +76,13 @@ class TrainStep:
             self.opt = torch.optim.Adam(self.params, lr=lr, amsgrad=True, capturable=True, foreach=True)
         self.static = {k: v.clone() for k, v in example_feats.items()}
         self.loss = torch.zeros((), dtype=torch.float32, device=dev)
+        # the global norm of the mean gradient before clipping, overwritten by every step (None: no clipping, no norm)
+        self.grad_norm: Optional[torch.Tensor] = None
+        if self.max_grad_norm is not None:
+            self.grad_norm = torch.zeros((), dtype=torch.float32, device=dev)
+            if self.fused_adam:
+                self.clip_coef = torch.ones((), dtype=torch.float32, device=dev)
+                self.norm_partial = torch.zeros(1024, dtype=torch.float64, device=dev)      # dfold_grad_norm's workspace
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.graph_error: Optional[str] = None
         verbose = os.environ.get("DFOLD_BENCH_VERBOSE", "0") == "1"
@@ -122,6 +138,8 @@ class TrainStep:
                             else:
                                 v.zero_()
             self.flat_grad.zero_()
+            if self.grad_norm is not None:
+                self.grad_norm.zero_()
         _kernels.invalidate_weight_cache()
         torch.cuda.synchronize()
 
@@ -155,15 +173,25 @@ class TrainStep:
         self.loss.copy_(loss.detach().float())
 
     def _adam(self, a: int, b: int, tick: bool):
-        _kernels.launch("dfold_adam_amsgrad", self.flat_param[a:b], self.flat_grad[a:b], self.exp_avg[a:b], self.exp_avg_sq[a:b],
-                        self.max_exp_avg_sq[a:b], b - a, self.step_count, 1 if tick else 0, self.lr, 0.9, 0.999, 1e-8,
-                        1.0 / self.world)
+        args = (self.flat_param[a:b], self.flat_grad[a:b], self.exp_avg[a:b], self.exp_avg_sq[a:b], self.max_exp_avg_sq[a:b],
+                b - a, self.step_count, 1 if tick else 0, self.lr, 0.9, 0.999, 1e-8, 1.0 / self.world)
+        if self.max_grad_norm is None:
+            _kernels.launch("dfold_adam_amsgrad", *args)
+        else:
+            _kernels.launch("dfold_adam_amsgrad_clip", *args, self.clip_coef)
 
     def optimizer_step(self):
         if self.opt is not None:
+            if self.max_grad_norm is not None:
+                # no host synchronisation with error_if_nonfinite=False, so this stays inside the captured graph
+                self.grad_norm.copy_(torch.nn.utils.clip_grad_norm_(self.params, self.max_grad_norm, foreach=True))
             self.opt.step()
             return
-        self._adam(0, self.flat_param.numel(), tick=True)
+        n = self.flat_param.numel()
+        if self.max_grad_norm is not None:
+            _kernels.launch("dfold_grad_norm", self.flat_grad, n, 1.0 / self.world, self.max_grad_norm, self.norm_partial,
+                            self.grad_norm, self.clip_coef)
+        self._adam(0, n, tick=True)
         _kernels.invalidate_weight_cache()                # the weights moved without touching their version counters
 
     def load(self, feats: Dict[str, torch.Tensor]):
@@ -230,3 +258,12 @@ class TrainStep:
                     v.copy_(model[k])
         _kernels.invalidate_weight_cache()          # no bf16 weight plane from before the load may be reused
         torch.cuda.synchronize()
+
+
+def _check_max_grad_norm(v) -> Optional[float]:
+    """None, or a positive number (``math.inf`` reports the norm without clipping, torch's idiom)."""
+    if v is None:
+        return None
+    if isinstance(v, bool) or not isinstance(v, numbers.Real) or not float(v) > 0:      # (NaN fails the comparison)
+        raise ValueError(f"max_grad_norm must be None or a positive number (math.inf: report the norm only), got {v!r}")
+    return float(v)

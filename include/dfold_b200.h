@@ -317,6 +317,21 @@ int dfold_featurize_window(const float* pos, const float* atom_mask, const long*
  * the gradient is multiplied by grad_scale on the fly (1 / world_size after a summing all-reduce). */
 int dfold_adam_amsgrad(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, long n,
                        float* step, int tick, float lr, float beta1, float beta2, float eps, float grad_scale, void* stream);
+/* Global-norm gradient clipping, the commented-out torch.nn.utils.clip_grad_norm_(model.parameters(), max_norm) of
+ * Experiment.update_fn (train_DFOLD_dynamics.py:665), with torch's norm_type=2 and error_if_nonfinite=False, applied to the
+ * data-parallel mean grad_scale * grad of a flat fp32 buffer of n elements (n % 4 == 0).  Writes the DEVICE scalars
+ * total = ||grad_scale * grad||_2 (clip_grad_norm_'s return value) and coef = min(max_norm / (total + 1e-6), 1) in fp32,
+ * NaN when total is NaN and 0 when it is inf, as torch computes them; the gradient is not modified.  The sum of squares
+ * runs in fp64 in an order that depends on n only (the same bits on every run, device and rank).  max_norm > 0;
+ * max_norm = inf gives coef 1 for any finite total.  partial: workspace of at least 1024 doubles. */
+int dfold_grad_norm(const float* grad, long n, float grad_scale, float max_norm, double* partial, float* total, float* coef,
+                    void* stream);
+/* dfold_adam_amsgrad on the clipped gradient (grad * grad_scale) * (*coef), the order of DDP's mean followed by
+ * clip_grad_norm_'s mul_(coef) (train_DFOLD_dynamics.py:665); coef is a DEVICE scalar (dfold_grad_norm's output), so no
+ * extra pass over the gradient is made.  *coef == 1 gives the bits of dfold_adam_amsgrad. */
+int dfold_adam_amsgrad_clip(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, long n,
+                            float* step, int tick, float lr, float beta1, float beta2, float eps, float grad_scale,
+                            const float* coef, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Evaluation metrics (csrc/metrics.cu), SURVEY.md 8 f6: the arithmetic of Experiment.eval_fn (train_DFOLD_dynamics.py:
