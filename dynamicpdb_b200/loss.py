@@ -1,8 +1,8 @@
 """Training loss of the DFOLDv2 score network on the device (SURVEY.md §8 f3).
 
 ``score_network_loss(model_out, batch, exp_conf)`` returns what ``Experiment.loss_fn`` returns after its model call
-(reference train_DFOLD_dynamics.py:1206-1400): ``(loss, aux_data)`` with the same keys, float64 like the reference (its
-loader hands float64 targets, which promotes the whole expression) and the same gradients.  Only the last trajectory
+(reference train_DFOLD_dynamics.py:1206-1400): ``(loss, aux_data)`` with the same keys and dtypes (float64: its loader hands
+float64 targets, which promotes every expression they enter) and the same gradients.  Only the last trajectory
 frame is trained on (:1222, :1248, :1312), so the whole loss is ONE kernel over the N residues of that frame
 (csrc/loss.cu) that also emits the gradients w.r.t. ``angles``, ``rot_score`` and the translation of ``rigids``; the
 backward pass only scales them.  ``t`` and ``rot_score_scaling`` are read on the device (no host synchronisation, so the
@@ -70,7 +70,10 @@ def score_network_loss(model_out: Dict[str, torch.Tensor], batch: Dict[str, torc
     out = _LossFn.apply(model_out["angles"], model_out["rot_score"], model_out["rigids"], fixed, consts)
     det = out.detach()
     rep = lambda v: v.reshape(1).repeat(batch_size)
-    aux = {"batch_train_loss": rep(det[7]), "batch_rot_loss": rep(det[4]), "batch_trans_loss": rep(det[5]),
-           "batch_torsion_loss": rep(det[6]), "total_loss": det[0], "rot_loss": det[1], "trans_loss": det[2],
+    # the translation term alone never meets a float64 target in the reference (:1241-1248): its two logging values keep
+    # the dtype of rigids_0 - rigids, float32 for the loader's batches
+    trans_dt = torch.promote_types(batch["rigids_0"].dtype, model_out["rigids"].dtype)
+    aux = {"batch_train_loss": rep(det[7]), "batch_rot_loss": rep(det[4]), "batch_trans_loss": rep(det[5]).to(trans_dt),
+           "batch_torsion_loss": rep(det[6]), "total_loss": det[0], "rot_loss": det[1], "trans_loss": det[2].to(trans_dt),
            "torsion_loss": det[3]}
     return out[0], aux

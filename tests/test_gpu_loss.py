@@ -30,7 +30,8 @@ def test_loss_kernel_matches_reference_golden(name):
     assert close(loss, gold["loss"], 1e-6)
     assert set(aux) == set(gold["aux"])
     for k in aux:
-        assert aux[k].shape == gold["aux"][k].shape and close(aux[k], gold["aux"][k], 1e-6), k
+        assert aux[k].shape == gold["aux"][k].shape and aux[k].dtype == gold["aux"][k].dtype, k
+        assert close(aux[k], gold["aux"][k], 1e-6), k
     for k, g in grads.items():
         ref = gold["grads"][k]
         ref = torch.zeros_like(g) if ref is None else ref
