@@ -52,10 +52,12 @@ def adam_param_groups(n_params: int, lr: float) -> list:
 
 
 def optimizer_state_dict(layout: FlatLayout, exp_avg: torch.Tensor, exp_avg_sq: torch.Tensor, max_exp_avg_sq: torch.Tensor,
-                         step: float, lr: float, indices: Optional[Sequence[int]] = None) -> dict:
+                         step: float, lr: float, indices: Optional[Sequence[int]] = None,
+                         initial_lr: Optional[float] = None) -> dict:
     """Host flat moment buffers -> the state_dict of ``torch.optim.Adam(net.parameters(), lr, amsgrad=True)``.  Every
     trained parameter gets an entry (``indices``: only those), each with its own float32 ``step`` tensor (torch increments
-    them one by one) and views of the flat buffers for the moments."""
+    them one by one) and views of the flat buffers for the moments.  ``initial_lr``: the optimizer's lr before a
+    learning-rate scheduler took over, which torch's LRScheduler adds to the param group."""
     keep = None if indices is None else set(indices)
     per = [views(layout, b) for b in (exp_avg, exp_avg_sq, max_exp_avg_sq)]
     state = {}
@@ -64,7 +66,10 @@ def optimizer_state_dict(layout: FlatLayout, exp_avg: torch.Tensor, exp_avg_sq: 
             continue
         state[i] = {"step": torch.tensor(float(step), dtype=torch.float32),
                     **{k: v[i] for k, v in zip(MOMENTS, per)}}
-    return {"state": state, "param_groups": adam_param_groups(len(layout.names), lr)}
+    groups = adam_param_groups(len(layout.names), lr)
+    if initial_lr is not None:
+        groups[0]["initial_lr"] = initial_lr
+    return {"state": state, "param_groups": groups}
 
 
 def strip_module_prefix(model: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
@@ -78,11 +83,13 @@ def _names(keys, limit=4):
     return ", ".join(map(str, keys[:limit])) + (f" and {len(keys) - limit} more" if len(keys) > limit else "")
 
 
-def check_state(sd: dict, layout: FlatLayout, model_shapes: Dict[str, torch.Size], lr: float
+def check_state(sd: dict, layout: FlatLayout, model_shapes: Dict[str, torch.Size], lr: float, schedule=None
                 ) -> Tuple[Dict[str, torch.Tensor], Optional[Dict[int, dict]], float]:
     """Validates a checkpoint dict against the step it is to be loaded into and returns (model tensors by the network's
     own names, optimizer state entries by parameter index or None for a weights-only load, the common step).  Raises
-    ValueError, naming the problem, for anything that would resume a different optimisation than the one saved."""
+    ValueError, naming the problem, for anything that would resume a different optimisation than the one saved.
+    ``schedule`` (train_step.AlphaFoldSchedule or None): the checkpoint's lr must be ``schedule.lr(step)``, the lr a
+    scheduler stepped once per optimizer step leaves in the param group, instead of ``lr``."""
     if not isinstance(sd, dict) or not isinstance(sd.get("model"), dict):
         raise ValueError("checkpoint has no 'model' state_dict")
     model = strip_module_prefix(sd["model"])
@@ -102,7 +109,7 @@ def check_state(sd: dict, layout: FlatLayout, model_shapes: Dict[str, torch.Size
         raise ValueError(f"checkpoint optimizer has {len(groups) if isinstance(groups, list) else 'no'} param groups; "
                          "the training step has a single one")
     g = groups[0]
-    if g.get("lr") != lr:
+    if schedule is None and g.get("lr") != lr:
         raise ValueError(f"checkpoint lr {g.get('lr')!r} differs from the training step's {lr!r}; the lr is part of the "
                          f"captured step: construct TrainStep(lr={g.get('lr')!r}) to resume this checkpoint")
     want = {"betas": ADAM_BETAS, "eps": ADAM_EPS, "weight_decay": 0, "amsgrad": True, "maximize": False}
@@ -131,7 +138,15 @@ def check_state(sd: dict, layout: FlatLayout, model_shapes: Dict[str, torch.Size
     if len(steps) > 1:
         raise ValueError(f"checkpoint optimizer state has different step counts {sorted(steps)}; the training step keeps "
                          "a single one")
-    return model, entries, steps.pop() if steps else 0.0
+    step = steps.pop() if steps else 0.0
+    if schedule is not None:
+        if not (step >= 0 and step == int(step)):
+            raise ValueError(f"checkpoint optimizer step {step!r} is not a whole number of steps")
+        want = schedule.lr(int(step))
+        if g.get("lr") != want:
+            raise ValueError(f"checkpoint lr {g.get('lr')!r} at step {int(step)} is not the learning-rate schedule's {want!r} "
+                             f"there: it was saved under a different schedule ({schedule})")
+    return model, entries, step
 
 
 def model_to_flat(layout: FlatLayout, model: Dict[str, torch.Tensor]) -> torch.Tensor:

@@ -603,14 +603,16 @@ namespace {
 __global__ void adam_tick_kernel(float* step) { *step += 1.f; }
 
 // kClip: the gradient is ((g * gscale) * *coef), the order of DDP's mean followed by clip_grad_norm_'s mul_(coef).
-template <bool kClip>
+// kDevLr: the learning rate is read from device memory (*dlr, written by lr_schedule_kernel) instead of the argument lr.
+template <bool kClip, bool kDevLr>
 __global__ void __launch_bounds__(256) adam_amsgrad_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                            float* __restrict__ v, float* __restrict__ vmax, long n4,
                                                            const float* __restrict__ step, float lr, float b1, float b2, float eps,
-                                                           float gscale, const float* __restrict__ coef) {
+                                                           float gscale, const float* __restrict__ coef,
+                                                           const float* __restrict__ dlr) {
     const float t = *step;
     const float bc1 = 1.f - powf(b1, t), bc2 = 1.f - powf(b2, t);
-    const float step_size = lr / bc1, inv_bc2_sqrt = 1.f / sqrtf(bc2);
+    const float step_size = (kDevLr ? *dlr : lr) / bc1, inv_bc2_sqrt = 1.f / sqrtf(bc2);
     const float c = kClip ? *coef : 1.f;
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
         float4 P = reinterpret_cast<float4*>(p)[i];
@@ -686,11 +688,31 @@ __global__ void __launch_bounds__(kNormThreads) grad_norm_finalize_kernel(const 
         *coef = (c > 1.f) ? 1.f : c;
     }
 }
+
+// ---------------------------------------------------------------------------------------------------
+// The AlphaFold learning-rate schedule (openfold/utils/lr_schedulers.py AlphaFoldLRScheduler.get_lr, the scheduler the
+// reference trainer imports, train_DFOLD_dynamics.py:56,652) at last_epoch = *step, the optimizer steps taken so far.  One
+// thread, evaluated in fp64 in Python's order with every operation rounded on its own (no contraction), then rounded to fp32
+// once: the value a Python float lr becomes when it is passed to the fp32 Adam.  The decay power decay ** e (integer e >= 1)
+// goes through pow as Python's float.__pow__ does.
+// ---------------------------------------------------------------------------------------------------
+__global__ void lr_schedule_kernel(const float* __restrict__ step, double base_lr, double max_lr, long warmup, long start,
+                                   long every, double decay, float* __restrict__ lr) {
+    const long s = (long)*step;
+    double v;
+    if (s <= warmup)
+        v = __dadd_rn(base_lr, __dmul_rn(__ddiv_rn((double)s, (double)warmup), max_lr));
+    else if (s > start)
+        v = __dmul_rn(max_lr, pow(decay, (double)((s - start) / every + 1)));
+    else
+        v = max_lr;
+    *lr = (float)v;
+}
 }  // namespace
 
 static int adam_launch(bool clip, float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq,
                        long n, float* step, int tick, float lr, float beta1, float beta2, float eps, float grad_scale,
-                       const float* coef, cudaStream_t st) {
+                       const float* coef, const float* dlr, cudaStream_t st) {
     if (tick) adam_tick_kernel<<<1, 1, 0, st>>>(step);            // chunked callers advance the step once per optimizer step
     const long n4 = n / 4;
     int dev = 0, sms = 0;
@@ -698,12 +720,15 @@ static int adam_launch(bool clip, float* param, const float* grad, float* exp_av
         sms = 132;
     const long cap = 16L * sms;                                     // 16 CTAs of 256 threads per SM, grid-stride beyond
     const int blocks = (int)(cdiv(n4, 256) < cap ? cdiv(n4, 256) : cap);
-    if (clip)
-        adam_amsgrad_kernel<true><<<blocks, 256, 0, st>>>(param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n4, step, lr, beta1,
-                                                          beta2, eps, grad_scale, coef);
-    else
-        adam_amsgrad_kernel<false><<<blocks, 256, 0, st>>>(param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n4, step, lr, beta1,
-                                                           beta2, eps, grad_scale, nullptr);
+#define DFOLD_ADAM(CLIP, DLR)                                                                                                  \
+    adam_amsgrad_kernel<CLIP, DLR><<<blocks, 256, 0, st>>>(param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n4, step, lr, beta1, \
+                                                           beta2, eps, grad_scale, coef, dlr)
+    if (dlr != nullptr) {
+        if (clip) DFOLD_ADAM(true, true); else DFOLD_ADAM(false, true);
+    } else {
+        if (clip) DFOLD_ADAM(true, false); else DFOLD_ADAM(false, false);
+    }
+#undef DFOLD_ADAM
     return check_launch("adam_amsgrad_kernel");
 }
 }  // namespace dfold
@@ -713,7 +738,7 @@ extern "C" int dfold_adam_amsgrad(float* param, const float* grad, float* exp_av
                                   float* step, int tick, float lr, float beta1, float beta2, float eps, float grad_scale, void* stream) {
     DFOLD_REQUIRE(n > 0 && n % 4 == 0, "dfold_adam_amsgrad: n must be a positive multiple of 4");
     return dfold::adam_launch(false, param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n, step, tick, lr, beta1, beta2, eps,
-                              grad_scale, nullptr, dfold::as_stream(stream));
+                              grad_scale, nullptr, nullptr, dfold::as_stream(stream));
 }
 
 extern "C" int dfold_adam_amsgrad_clip(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq,
@@ -722,7 +747,29 @@ extern "C" int dfold_adam_amsgrad_clip(float* param, const float* grad, float* e
     DFOLD_REQUIRE(n > 0 && n % 4 == 0, "dfold_adam_amsgrad_clip: n must be a positive multiple of 4");
     DFOLD_REQUIRE(coef != nullptr, "dfold_adam_amsgrad_clip: null coefficient");
     return dfold::adam_launch(true, param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n, step, tick, lr, beta1, beta2, eps,
-                              grad_scale, coef, dfold::as_stream(stream));
+                              grad_scale, coef, nullptr, dfold::as_stream(stream));
+}
+
+// lr: DEVICE fp32 scalar; coef: nullable (no clipping).
+extern "C" int dfold_adam_amsgrad_dlr(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq,
+                                      long n, float* step, int tick, const float* lr, float beta1, float beta2, float eps,
+                                      float grad_scale, const float* coef, void* stream) {
+    DFOLD_REQUIRE(n > 0 && n % 4 == 0, "dfold_adam_amsgrad_dlr: n must be a positive multiple of 4");
+    DFOLD_REQUIRE(lr != nullptr, "dfold_adam_amsgrad_dlr: null learning rate");
+    return dfold::adam_launch(coef != nullptr, param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n, step, tick, 0.f, beta1, beta2,
+                              eps, grad_scale, coef, lr, dfold::as_stream(stream));
+}
+
+extern "C" int dfold_lr_schedule(const float* step, double base_lr, double max_lr, long warmup_no_steps,
+                                 long start_decay_after_n_steps, long decay_every_n_steps, double decay_factor, float* lr,
+                                 void* stream) {
+    DFOLD_REQUIRE(step != nullptr && lr != nullptr, "dfold_lr_schedule: null step or lr");
+    DFOLD_REQUIRE(warmup_no_steps > 0 && decay_every_n_steps > 0 && warmup_no_steps <= start_decay_after_n_steps,
+                  "dfold_lr_schedule: needs 0 < warmup_no_steps <= start_decay_after_n_steps and decay_every_n_steps > 0");
+    DFOLD_REQUIRE(max_lr > 0.0 && max_lr < INFINITY, "dfold_lr_schedule: max_lr must be positive and finite");
+    dfold::lr_schedule_kernel<<<1, 1, 0, dfold::as_stream(stream)>>>(step, base_lr, max_lr, warmup_no_steps,
+                                                                     start_decay_after_n_steps, decay_every_n_steps, decay_factor, lr);
+    return dfold::check_launch("lr_schedule_kernel");
 }
 
 // partial: workspace of at least 1024 doubles.

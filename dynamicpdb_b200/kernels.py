@@ -59,6 +59,8 @@ _SIGS = {
     "dfold_adam_amsgrad": "pppppl" + "pi" + "fffff" + "p",
     "dfold_adam_amsgrad_clip": "pppppl" + "pi" + "fffff" + "pp",
     "dfold_grad_norm": "plff" + "ppp" + "p",
+    "dfold_adam_amsgrad_dlr": "pppppl" + "pi" + "p" + "ffff" + "pp",
+    "dfold_lr_schedule": "p" + "dd" + "lll" + "d" + "pp",
     "dfold_featurize_window": "pppppp" + "ii" + "pppp" + "p",
     "dfold_loss_fwd": "pppppppppppp" + "ii" + "dddd" + "ii" + "pppp" + "p",
     "dfold_quat_mul_fwd": "ppplip",

@@ -332,6 +332,22 @@ int dfold_grad_norm(const float* grad, long n, float grad_scale, float max_norm,
 int dfold_adam_amsgrad_clip(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, long n,
                             float* step, int tick, float lr, float beta1, float beta2, float eps, float grad_scale,
                             const float* coef, void* stream);
+/* dfold_adam_amsgrad (coef NULL) or dfold_adam_amsgrad_clip (coef non-NULL) with the learning rate read from the DEVICE
+ * fp32 scalar *lr (dfold_lr_schedule's output), so a captured step follows a schedule.  The same kernel: *lr equal to
+ * fp32(x) gives the bits of the by-value call with lr = x. */
+int dfold_adam_amsgrad_dlr(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, long n,
+                           float* step, int tick, const float* lr, float beta1, float beta2, float eps, float grad_scale,
+                           const float* coef, void* stream);
+/* The learning rate of AlphaFoldLRScheduler.get_lr (openfold/utils/lr_schedulers.py:64-82, imported by the reference
+ * trainer, train_DFOLD_dynamics.py:56,652) at last_epoch = s = *step (the DEVICE step counter of dfold_adam_amsgrad, read
+ * before the step's tick), written to the DEVICE fp32 scalar *lr by one thread:
+ *   base_lr + s / warmup_no_steps * max_lr                                                          s <= warmup_no_steps
+ *   max_lr * decay_factor ** ((s - start_decay_after_n_steps) // decay_every_n_steps + 1)       s > start_decay_after_n_steps
+ *   max_lr                                                                                         otherwise
+ * evaluated in fp64 as Python evaluates it, then rounded to fp32 once.  Needs 0 < warmup_no_steps <=
+ * start_decay_after_n_steps, decay_every_n_steps > 0 and a finite max_lr > 0. */
+int dfold_lr_schedule(const float* step, double base_lr, double max_lr, long warmup_no_steps, long start_decay_after_n_steps,
+                      long decay_every_n_steps, double decay_factor, float* lr, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Evaluation metrics (csrc/metrics.cu), SURVEY.md 8 f6: the arithmetic of Experiment.eval_fn (train_DFOLD_dynamics.py:
