@@ -33,10 +33,16 @@ __device__ __forceinline__ uint32_t split_pack(float x) {
     return ((uint32_t)__bfloat16_as_ushort(h) << 16) | (uint32_t)__bfloat16_as_ushort(l);
 }
 
+// The ReLU gate of a layer at element i: gate > 0, or (gate - gate_sub) > 0 for a residual layer whose gate is its output
+// minus the residual.  The fp32 subtraction rounds as torch's would, so the gate opens on exactly the same elements.
+__device__ __forceinline__ bool gate_open(const float* __restrict__ gate, const float* __restrict__ gate_sub, long i) {
+    return (gate_sub ? gate[i] - gate_sub[i] : gate[i]) > 0.f;
+}
+
 // x[R, C] (row stride ld) -> hi/lo [R, ldo] and optionally transposed hi_t/lo_t [C, ldt].
-// Optional: relu on the input, a gate (x *= gate > 0).  The column sums of the (gated) input come from colsum_kernel.
+// Optional: relu on the input, a gate (x *= gate_open).  The column sums of the (gated) input come from colsum_kernel.
 __global__ void split2d_kernel(const float* __restrict__ x, long R, long C, long ld, int pre_relu,
-                               const float* __restrict__ gate, long ldg,
+                               const float* __restrict__ gate, const float* __restrict__ gate_sub, long ldg,
                                uint16_t* __restrict__ hi, uint16_t* __restrict__ lo, long ldo, long cpad,
                                uint16_t* __restrict__ hit, uint16_t* __restrict__ lot, long ldt, long rpad) {
     __shared__ uint32_t tile[32][33];
@@ -49,7 +55,7 @@ __global__ void split2d_kernel(const float* __restrict__ x, long R, long C, long
         if (r < R && c < C) {
             v = x[r * ld + c];
             if (pre_relu) v = fmaxf(v, 0.f);
-            if (gate) v = (gate[r * ldg + c] > 0.f) ? v : 0.f;
+            if (gate) v = gate_open(gate, gate_sub, r * ldg + c) ? v : 0.f;
         }
         const uint32_t pk = split_pack(v);
         tile[ty + i * 8][tx] = pk;
@@ -75,7 +81,8 @@ __global__ void split2d_kernel(const float* __restrict__ x, long R, long C, long
 // Row-major fast path of split2d (no transposed planes, no column sums, 16-byte aligned rows): one thread = four consecutive
 // columns, float4 in, 8 bytes of each plane out.
 __global__ void __launch_bounds__(256) split2d_vec_kernel(const float* __restrict__ x, long R, long C, long ld, int pre_relu,
-                                                          const float* __restrict__ gate, long ldg, uint16_t* __restrict__ hi,
+                                                          const float* __restrict__ gate, const float* __restrict__ gate_sub,
+                                                          long ldg, uint16_t* __restrict__ hi,
                                                           uint16_t* __restrict__ lo, long ldo, long c4n) {
     const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= R * c4n) return;
@@ -85,7 +92,11 @@ __global__ void __launch_bounds__(256) split2d_vec_kernel(const float* __restric
         const float4 t = *reinterpret_cast<const float4*>(x + r * ld + c);
         v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
         if (gate) {
-            const float4 g = *reinterpret_cast<const float4*>(gate + r * ldg + c);
+            float4 g = *reinterpret_cast<const float4*>(gate + r * ldg + c);
+            if (gate_sub) {
+                const float4 s = *reinterpret_cast<const float4*>(gate_sub + r * ldg + c);
+                g.x -= s.x; g.y -= s.y; g.z -= s.z; g.w -= s.w;
+            }
             v[0] = g.x > 0.f ? v[0] : 0.f; v[1] = g.y > 0.f ? v[1] : 0.f; v[2] = g.z > 0.f ? v[2] : 0.f; v[3] = g.w > 0.f ? v[3] : 0.f;
         }
     } else {
@@ -93,7 +104,7 @@ __global__ void __launch_bounds__(256) split2d_vec_kernel(const float* __restric
         for (int k = 0; k < 4; ++k)
             if (c + k < C) {
                 v[k] = x[r * ld + c + k];
-                if (gate) v[k] = (gate[r * ldg + c + k] > 0.f) ? v[k] : 0.f;
+                if (gate) v[k] = gate_open(gate, gate_sub, r * ldg + c + k) ? v[k] : 0.f;
             }
     }
     if (pre_relu) {                     // relu and the gate commute: relu(gate ? v : 0) == gate ? relu(v) : 0
@@ -382,7 +393,8 @@ __global__ void gln_bwd_apply_kernel(const float* __restrict__ x, const float* _
 // Column sums over all rows in one fixed order (no atomics, so the result is the same from run to run): one CTA per 32
 // columns, 32 row lanes; lane r adds rows r, r + 32, ... in turn, then the 32 lane sums are added in lane order.
 __global__ void __launch_bounds__(1024) colsum_kernel(const float* __restrict__ x, long R, long C, long ld, int pre_relu,
-                                                      const float* __restrict__ gate, long ldg, float* __restrict__ colsum) {
+                                                      const float* __restrict__ gate, const float* __restrict__ gate_sub, long ldg,
+                                                      float* __restrict__ colsum) {
     __shared__ float red[32][33];
     const int tx = threadIdx.x, ty = threadIdx.y;
     const long c = (long)blockIdx.x * 32 + tx;
@@ -391,7 +403,7 @@ __global__ void __launch_bounds__(1024) colsum_kernel(const float* __restrict__ 
         for (long r = ty; r < R; r += 32) {
             float v = x[r * ld + c];
             if (pre_relu) v = fmaxf(v, 0.f);
-            if (gate) v = (gate[r * ldg + c] > 0.f) ? v : 0.f;
+            if (gate) v = gate_open(gate, gate_sub, r * ldg + c) ? v : 0.f;
             s += v;
         }
     }
@@ -488,10 +500,10 @@ extern "C" int dfold_capture_id(void* stream, unsigned long long* id_out) {
     return 0;
 }
 
-// hi/lo: [R][ldo], columns [C, cpad) zero-filled.  hi_t/lo_t: [C][ldt], columns [R, rpad) zero-filled.
-extern "C" int dfold_split2d(const float* x, long R, long C, long ld, int pre_relu, const float* gate, long ldg,
-                             uint16_t* hi, uint16_t* lo, long ldo, long cpad, uint16_t* hi_t, uint16_t* lo_t, long ldt, long rpad,
-                             float* colsum, void* stream) {
+namespace {
+int split2d(const float* x, long R, long C, long ld, int pre_relu, const float* gate, const float* gate_sub, long ldg,
+            uint16_t* hi, uint16_t* lo, long ldo, long cpad, uint16_t* hi_t, uint16_t* lo_t, long ldt, long rpad,
+            float* colsum, void* stream) {
     DFOLD_REQUIRE(R > 0 && C > 0, "dfold_split2d: empty input");
     DFOLD_REQUIRE((hi == nullptr) == (lo == nullptr) && (hi_t == nullptr) == (lo_t == nullptr), "dfold_split2d: hi/lo must come in pairs");
     DFOLD_REQUIRE(hi == nullptr || (cpad >= C && ldo >= cpad), "dfold_split2d: need C <= cpad <= ldo");
@@ -500,20 +512,38 @@ extern "C" int dfold_split2d(const float* x, long R, long C, long ld, int pre_re
     const long cols = (hi && cpad > C) ? cpad : C;
     const long rows = (hi_t && rpad > R) ? rpad : R;
     if (colsum) {
-        colsum_kernel<<<(unsigned)cdiv(C, 32), dim3(32, 32), 0, as_stream(stream)>>>(x, R, C, ld, pre_relu, gate, ldg, colsum);
+        colsum_kernel<<<(unsigned)cdiv(C, 32), dim3(32, 32), 0, as_stream(stream)>>>(x, R, C, ld, pre_relu, gate, gate_sub, ldg, colsum);
         if (check_launch("colsum_kernel")) return 1;
     }
     if (!hi && !hi_t) return 0;         // column sums only (a bias gradient without operand planes)
     if (hi && !hi_t && (ld & 3) == 0 && (ldo & 3) == 0 && (cpad & 3) == 0 && (!gate || (ldg & 3) == 0) &&
-        ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(gate)) & 15) == 0 &&
+        ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(gate) | reinterpret_cast<uintptr_t>(gate_sub)) & 15) == 0 &&
         ((reinterpret_cast<uintptr_t>(hi) | reinterpret_cast<uintptr_t>(lo)) & 7) == 0) {
         const long c4n = cpad / 4, n = R * c4n;
-        split2d_vec_kernel<<<(unsigned)cdiv(n, 256), 256, 0, as_stream(stream)>>>(x, R, C, ld, pre_relu, gate, ldg, hi, lo, ldo, c4n);
+        split2d_vec_kernel<<<(unsigned)cdiv(n, 256), 256, 0, as_stream(stream)>>>(x, R, C, ld, pre_relu, gate, gate_sub, ldg, hi, lo,
+                                                                                   ldo, c4n);
         return check_launch("split2d_vec_kernel");
     }
     dim3 grid((unsigned)cdiv(cols, 32), (unsigned)cdiv(rows, 32));
-    split2d_kernel<<<grid, dim3(32, 8), 0, as_stream(stream)>>>(x, R, C, ld, pre_relu, gate, ldg, hi, lo, ldo, cpad, hi_t, lo_t, ldt, rpad);
+    split2d_kernel<<<grid, dim3(32, 8), 0, as_stream(stream)>>>(x, R, C, ld, pre_relu, gate, gate_sub, ldg, hi, lo, ldo, cpad,
+                                                                hi_t, lo_t, ldt, rpad);
     return check_launch("split2d_kernel");
+}
+}  // namespace
+
+// hi/lo: [R][ldo], columns [C, cpad) zero-filled.  hi_t/lo_t: [C][ldt], columns [R, rpad) zero-filled.
+extern "C" int dfold_split2d(const float* x, long R, long C, long ld, int pre_relu, const float* gate, long ldg,
+                             uint16_t* hi, uint16_t* lo, long ldo, long cpad, uint16_t* hi_t, uint16_t* lo_t, long ldt, long rpad,
+                             float* colsum, void* stream) {
+    return split2d(x, R, C, ld, pre_relu, gate, nullptr, ldg, hi, lo, ldo, cpad, hi_t, lo_t, ldt, rpad, colsum, stream);
+}
+
+// dfold_split2d with the gate of a residual layer: an element passes where (out - residual) > 0 (both [R][ldg]).
+extern "C" int dfold_split2d_residual_gate(const float* x, long R, long C, long ld, int pre_relu, const float* out,
+                                           const float* residual, long ldg, uint16_t* hi, uint16_t* lo, long ldo, long cpad,
+                                           uint16_t* hi_t, uint16_t* lo_t, long ldt, long rpad, float* colsum, void* stream) {
+    DFOLD_REQUIRE(out != nullptr && residual != nullptr, "dfold_split2d_residual_gate: out and residual are required");
+    return split2d(x, R, C, ld, pre_relu, out, residual, ldg, hi, lo, ldo, cpad, hi_t, lo_t, ldt, rpad, colsum, stream);
 }
 
 extern "C" int dfold_conv_weight_prep(const float* w, int O, int I, int T, uint16_t* f_hi, uint16_t* f_lo, long ldi,

@@ -10,6 +10,7 @@ pointers, appends the current stream and raises with the library's message on fa
 torch is used for: device memory (``torch.empty``), streams, autograd bookkeeping, and trivial view / elementwise
 glue (cat, slicing, SiLU on tiny tensors, masks).
 """
+import contextlib
 import ctypes
 import functools
 import os
@@ -30,6 +31,7 @@ _SIGS = {
     "dfold_debug_gemm_stats": "p",
     "dfold_debug_ipa_stats": "p",
     "dfold_split2d": "plllipl" + "ppll" + "ppll" + "pp",
+    "dfold_split2d_residual_gate": "plllippl" + "ppll" + "ppll" + "pp",
     "dfold_conv_weight_prep": "piii" + "ppl" + "ppl" + "p",
     "dfold_taps_to_param": "piiipip",
     "dfold_sgemm": "pllll" * 4 + "p" + "iiiii" + "ff" + "iii" + "p",
@@ -109,8 +111,14 @@ LAUNCH_COUNT = 0
 # straight into the parameter's existing .grad buffer and autograd receives None: the ConvNet is shared by the four blocks
 # (ipa_pytorch_dynamic.py:749,863), so the default path costs three 82 MB add passes per weight and step.
 GRAD_ACCUMULATE_INPLACE = False
-# optional per-launch timing: when PROFILE is a list, timed(...) appends (name, work, start_event, end_event)
+# optional per-launch timing: when PROFILE is a list, timed(...) appends (name, work, start_event, end_event).  Every launch
+# then stays on the current stream, so each event pair times one kernel running alone.
 PROFILE = None
+# The in-place convolution weight gradients run on one side stream per device (created on first use), overlapping the rest
+# of the backward: nothing in the backward reads them.  _SIDE_HELD keeps the tensors that work reads alive until
+# join_side_stream(); the caching allocator would otherwise hand their memory to the current stream while it is still read.
+_SIDE_STREAMS = {}
+_SIDE_HELD = {}
 
 
 _PASS = frozenset((int, float, type(None), ctypes.c_void_p))
@@ -147,6 +155,29 @@ class _timed:
             self.e1.record()
             PROFILE.append((self.name, self.work, self.e0, self.e1, self.tag))
         return False
+
+
+@contextlib.contextmanager
+def _on_side_stream(dev, held):
+    """Run the enclosed launches on ``dev``'s side stream, after all work queued so far on the current stream.  ``held``:
+    tensors from the current stream's memory that they read, kept alive until join_side_stream()."""
+    side = _SIDE_STREAMS.get(dev.index)
+    if side is None:
+        side = _SIDE_STREAMS[dev.index] = torch.cuda.Stream(device=dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
+    _SIDE_HELD.setdefault(dev.index, []).extend(held)
+    with torch.cuda.stream(side):
+        yield
+
+
+def join_side_stream():
+    """Make the current stream wait for the work queued on the side streams and release the tensors it read.  Call it after
+    a backward that accumulated in place (GRAD_ACCUMULATE_INPLACE) and before the gradient buffer is read; under CUDA-graph
+    capture it joins the side branch back into the captured stream."""
+    for idx, held in list(_SIDE_HELD.items()):
+        torch.cuda.current_stream(idx).wait_stream(_SIDE_STREAMS[idx])
+        held.clear()
+    _SIDE_HELD.clear()
 
 
 def _ptr(t: Optional[torch.Tensor], offset: int = 0):
@@ -219,10 +250,11 @@ def _sgemm(A, a_off, a_rs, a_cs, a_bs, a_bs2, B, b_off, b_rs, b_cs, b_bs, b_bs2,
            bias, batch, batch2, M, N, K, alpha, beta, act, pre_relu, 1)
 
 
-def _split2d(x2: torch.Tensor, *, pre_relu=False, gate=None, want=True, want_t=False, colsum=None,
+def _split2d(x2: torch.Tensor, *, pre_relu=False, gate=None, gate_sub=None, want=True, want_t=False, colsum=None,
              t_out=None, t_ld=None, t_off=0, rpad=None):
     """x2 [R, C] fp32 contiguous -> (hi, lo) [R, C8] and / or transposed planes [C, R8] (or into ``t_out``); ``colsum``
-    ([C], zeroed) receives the column sums of the gated input."""
+    ([C], zeroed) receives the column sums of the gated input.  The gate passes x2 where ``gate > 0``, or with
+    ``gate_sub`` (same strides as ``gate``) where ``gate - gate_sub > 0``."""
     R, C = x2.shape
     hi = lo = hit = lot = None
     c8 = _pad8(C)
@@ -240,8 +272,13 @@ def _split2d(x2: torch.Tensor, *, pre_relu=False, gate=None, want=True, want_t=F
         else:
             hit, lot = t_out
             ldt, rp = t_ld, rpad
-    launch("dfold_split2d", x2, R, C, x2.stride(0), int(pre_relu), gate, gate.stride(0) if gate is not None else 0,
-           hi, lo, c8, c8, _ptr(hit, t_off), _ptr(lot, t_off), ldt, rp, colsum)
+    ldg = gate.stride(0) if gate is not None else 0
+    if gate_sub is None:
+        launch("dfold_split2d", x2, R, C, x2.stride(0), int(pre_relu), gate, ldg,
+               hi, lo, c8, c8, _ptr(hit, t_off), _ptr(lot, t_off), ldt, rp, colsum)
+    else:
+        launch("dfold_split2d_residual_gate", x2, R, C, x2.stride(0), int(pre_relu), gate, gate_sub, ldg,
+               hi, lo, c8, c8, _ptr(hit, t_off), _ptr(lot, t_off), ldt, rp, colsum)
     return (hi, lo), (hit, lot)
 
 
@@ -374,15 +411,12 @@ class _LinearFn(Function):
         M_, K_ = ctx.mk
         N_ = w.shape[0]
         g = _f32c(dy.reshape(M_, N_))
-        gate = None
-        if act == "relu":
-            gate = out if r2 is None else (out - r2)
         dres = dy.reshape(rshape) if rshape else None
         need_x, need_w, need_b = ctx.needs_input_grad[0], ctx.needs_input_grad[1], has_b and ctx.needs_input_grad[2]
         dx = dw = db = None
         if tc:
             db_buf = torch.zeros(N_, dtype=torch.float32, device=g.device) if need_b else None
-            (g_hi, g_lo), _ = _split2d(g, gate=gate, want=need_x or need_w, colsum=db_buf)
+            (g_hi, g_lo), _ = _split2d(g, gate=out, gate_sub=r2, want=need_x or need_w, colsum=db_buf)
             db = db_buf
             if need_x:
                 _, _, wt_hi, wt_lo = _linear_planes(w)
@@ -392,8 +426,8 @@ class _LinearFn(Function):
                 dw = torch.empty((N_, K_), dtype=torch.float32, device=g.device)
                 _gemm_wgrad((g_hi, g_lo), N_, g_hi.shape[1], (a_hi, a_lo), K_, a_hi.shape[1], 1, M_, 1, 1, dw, K_)
         else:
-            if gate is not None:
-                g = g * (gate > 0)
+            if out is not None:
+                g = g * ((out if r2 is None else out - r2) > 0)
             wf = _f32c(w)
             if need_x:
                 dx = torch.empty((M_, K_), dtype=torch.float32, device=g.device)
@@ -465,31 +499,44 @@ class _Conv5x5Fn(Function):
         Co, _, kh, kw = w.shape
         Fo = F_ - crop
         g = _f32c(dy.reshape(Fo * N_, Co))
-        gate = None
-        if relu:
-            gate = out if r2 is None else (out - r2)
         need_x, need_w, need_b = ctx.needs_input_grad[0], ctx.needs_input_grad[1], has_b and ctx.needs_input_grad[2]
         dx = dw = db = None
         db_buf = torch.zeros(Co, dtype=torch.float32, device=g.device) if need_b else None
-        (g_hi, g_lo), _ = _split2d(g, gate=gate, want=need_x or need_w, colsum=db_buf)
+        (g_hi, g_lo), _ = _split2d(g, gate=out, gate_sub=r2, want=need_x or need_w, colsum=db_buf)
         db = db_buf
+        acc = None
+        if need_w and GRAD_ACCUMULATE_INPLACE and ctx.w_param is not None:
+            acc = ctx.w_param.grad
+            if not (acc is not None and acc.dtype == torch.float32 and acc.is_contiguous() and acc.shape == w.shape
+                    and acc.device == g.device):
+                acc = None
+        wgrad = lambda out_, add: _conv_wgrad(g_hi, g_lo, x_hi, x_lo, Co, Ci, kh, kw, F_, Fo, N_, crop, out_, add)
+        side = acc is not None and PROFILE is None
+        if side:
+            # the weight gradient only adds into the parameter's .grad: it overlaps the data gradient and the rest of the
+            # backward, which never read it
+            with _on_side_stream(g.device, (g_hi, g_lo, x_hi, x_lo)):
+                wgrad(acc, 1)
         if need_x:
             _, _, d_hi, d_lo = _conv_planes(w)
             dx = torch.empty((F_ * N_, Ci), dtype=torch.float32, device=g.device)
             _gemm(g_hi, g_lo, Fo, N_, Co, Co, d_hi, d_lo, Ci, d_hi.shape[2], kh, kw, dx, Ci, None, None, 0, 1.0, 0.0, 0,
                   F_out=F_, f_start=-crop)
             dx = dx.reshape(F_, N_, Ci)
-        if need_w:
-            taps = torch.empty((kh * kw, Co, Ci), dtype=torch.float32, device=g.device)
-            _gemm_wgrad((g_hi, g_lo), Co, Co, (x_hi, x_lo), Ci, Ci, Fo, N_, kh, kw, taps, Ci, Fb=F_, b_f_add=crop)
-            wp = ctx.w_param
-            acc = wp.grad if (GRAD_ACCUMULATE_INPLACE and wp is not None) else None
-            if acc is not None and acc.dtype == torch.float32 and acc.is_contiguous() and acc.shape == w.shape and acc.device == g.device:
-                launch("dfold_taps_to_param", taps, Co, Ci, kh * kw, acc, 1)
-            else:
-                dw = torch.empty((Co, Ci, kh, kw), dtype=torch.float32, device=g.device)
-                launch("dfold_taps_to_param", taps, Co, Ci, kh * kw, dw, 0)
+        if acc is not None and not side:
+            wgrad(acc, 1)
+        elif need_w and acc is None:
+            dw = torch.empty((Co, Ci, kh, kw), dtype=torch.float32, device=g.device)
+            wgrad(dw, 0)
         return dx, dw, db, None, (dy if has_r else None), None
+
+
+def _conv_wgrad(g_hi, g_lo, x_hi, x_lo, Co, Ci, kh, kw, F_, Fo, N_, crop, out, add):
+    """Weight gradient of the convolution: the per-tap GEMMs into a [taps, Co, Ci] scratch (allocated on the current
+    stream), then added into (add=1) or written to (add=0) ``out`` [Co, Ci, kh, kw]."""
+    taps = torch.empty((kh * kw, Co, Ci), dtype=torch.float32, device=out.device)
+    _gemm_wgrad((g_hi, g_lo), Co, Co, (x_hi, x_lo), Ci, Ci, Fo, N_, kh, kw, taps, Ci, Fb=F_, b_f_add=crop)
+    launch("dfold_taps_to_param", taps, Co, Ci, kh * kw, out, add)
 
 
 def conv5x5(x, weight, bias=None, relu: bool = True, residual=None, crop: int = 0):

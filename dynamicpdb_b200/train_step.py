@@ -175,7 +175,10 @@ class TrainStep:
             try:
                 _kernels.invalidate_weight_cache()
                 g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
+                # captured at a higher priority than the side stream of the convolution weight gradients (kernels.py): the
+                # block scheduler then serves the backward's critical path first, and the weight gradients fill the SMs
+                # it leaves idle instead of holding them while it waits
+                with torch.cuda.graph(g, stream=torch.cuda.Stream(device=dev, priority=-1)):
                     self._eager()
                 self.graph = g
             except Exception as e:                       # noqa: BLE001  (report and fall back to eager launches)
@@ -225,6 +228,9 @@ class TrainStep:
                 loss.backward()                      # AccumulateGrad adds into the param.grad views of the flat buffer
             finally:
                 _kernels.GRAD_ACCUMULATE_INPLACE = prev
+                # the convolution weight gradients added on the side stream are complete before anything reads the buffer;
+                # joining once per window also frees the activation planes they read before the next window's forward
+                _kernels.join_side_stream()
             if i == 0:
                 self.loss.copy_(loss.detach().float())
             else:

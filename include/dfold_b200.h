@@ -46,6 +46,13 @@ int dfold_split2d(const float* x, long R, long C, long ld, int pre_relu, const f
                   uint16_t* hi, uint16_t* lo, long ldo, long cpad,
                   uint16_t* hi_t, uint16_t* lo_t, long ldt, long rpad, float* colsum, void* stream);
 
+/* dfold_split2d with the ReLU gate of a residual layer y = relu(...) + residual: x passes where the fp32 difference
+ * out - residual is > 0 (out and residual both [R] rows of stride ldg, neither nullable).  Planes and column sums are
+ * those dfold_split2d gives for gate = out - residual computed beforehand. */
+int dfold_split2d_residual_gate(const float* x, long R, long C, long ld, int pre_relu, const float* out,
+                                const float* residual, long ldg, uint16_t* hi, uint16_t* lo, long ldo, long cpad,
+                                uint16_t* hi_t, uint16_t* lo_t, long ldt, long rpad, float* colsum, void* stream);
+
 /* Conv weight w[O][I][T] (the reference layout [C_out, C_in, 5, 5], T = 25) ->
  *   forward planes  f_hi/f_lo [T][O][ldi]           (K = input channel)
  *   dgrad planes    d_hi/d_lo [T][I][ldo], tap order flipped (nullable pair)
