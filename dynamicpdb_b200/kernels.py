@@ -320,11 +320,16 @@ def _cache_get(kind, w: torch.Tensor, build):
     # graph's entry would read planes only that other graph refreshes.  Within one capture the same weight is split
     # once: the entry keyed with this capture's id serves the remaining call sites.
     val = build()
-    if len(_WCACHE) > 512:
-        for k in [k for k, e in _WCACHE.items() if e[0]() is None]:
-            del _WCACHE[k]
-    _WCACHE[key] = (weakref.ref(w), stamp, val)
+    # the planes go when the weight does (a preset-A model holds 2.6 GB of them), not when the cache next fills up
+    _WCACHE[key] = (weakref.ref(w, lambda ref, key=key: _cache_drop(key, ref)), stamp, val)
     return val
+
+
+def _cache_drop(key, ref):
+    """Weakref callback: forget the entry of a weight that died (unless a newer entry has taken its key)."""
+    ent = _WCACHE.get(key)
+    if ent is not None and ent[0] is ref:
+        del _WCACHE[key]
 
 
 def _linear_planes(w: torch.Tensor):
