@@ -12,8 +12,8 @@ cannot keep one GPU fed, let alone eight.  Here:
   stream (``select_random_samples`` / ``select_first_samples``, :164-190);
 * ``featurize_window`` computes ``rigids_0`` and the torsion features of a window with one kernel on the device
   (csrc/featurize.cu), from the fp32 coordinates of the ``frame_time`` selected frames only;
-* ``WindowPrefetcher`` overlaps the next window's slicing and host->device copy (side stream, pinned staging buffers)
-  with the current training step;
+* ``WindowPrefetcher`` overlaps the next window's host->device copy (side stream, straight from the store's pinned
+  memory) with the current training step;
 * given a diffuser (``score_epilogue.SE3ScoreDiffuser``), the same side stream also noises the window (:332-349):
   in training ``t ~ U(min_t, 1)`` is drawn on the device and ``forward_marginal`` (csrc/diffuse.cu) adds ``t``,
   ``rigids_t``, both scores and both score scalings; in evaluation ``t = 1`` and ``sample_ref`` gives ``rigids_t``.
@@ -71,7 +71,9 @@ class TrajectoryStore:
         return t.pin_memory() if self.pin else t
 
     def protein(self, atlas_npz: str, force_path: str, vel_path: str, embed_path: str) -> Dict[str, torch.Tensor]:
-        """Load (once) and cache one protein: the file naming follows Dfold_data_loader_dynamic.py:194-198."""
+        """Load (once) and cache one protein: the file naming follows Dfold_data_loader_dynamic.py:194-198.  The frames
+        kept are the first ``keep_first`` (training windows) and the ones up to the end of the evaluation window, which
+        starts at ``fix_sample_start`` whatever ``keep_first`` is (:214-218)."""
         if atlas_npz in self._cache:
             return self._cache[atlas_npz]
         with np.load(atlas_npz, allow_pickle=True) as zf:
@@ -83,6 +85,8 @@ class TrajectoryStore:
         with np.load(embed_path) as ef:
             emb = {k: ef[k] for k in ("node_repr", "edge_repr")}
         kf = self.keep_first
+        if kf is not None:
+            kf = max(kf, self.fix_start + self.frame_time * self.step)
         ent = {
             "atom37": self._pin(z["all_atom_positions"][:kf], torch.float32),                 # [T,N,37,3]
             "force": self._pin(np.asarray(force)[:kf], torch.float64),                        # [T,N,3] (the loader's dtype)
@@ -97,20 +101,35 @@ class TrajectoryStore:
         return ent
 
     def window_index(self, n_frames: int, training: bool) -> slice:
-        """The reference's window arithmetic (:164-190), drawing from numpy's global stream exactly as it does."""
+        """The reference's window arithmetic (:164-190, :214-218), drawing from numpy's global stream exactly as it does.
+        ``n_frames`` is the number of frames ``protein`` kept.  Training windows lie in the first ``keep_first`` frames;
+        evaluation windows start at ``fix_sample_start`` and may reach past them.  An evaluation window shorter than
+        ``frame_time`` raises (the reference raises when fewer than ``frame_time`` frames follow the start)."""
         t, k = self.frame_time, self.step
         if training:
-            if t > n_frames:
+            n = n_frames if self.keep_first is None else min(n_frames, self.keep_first)
+            if t > n:
                 raise ValueError("t cannot be greater than the number of samples")
-            start = np.random.randint(0, n_frames - t * k + 1)
+            start = np.random.randint(0, n - t * k + 1)
         else:
             start = self.fix_start
+            n = n_frames - start
+            if t > n:
+                raise ValueError("t cannot be greater than the number of samples")
+            if (t - 1) * k >= n:
+                raise ValueError(f"the evaluation window ({t} frames every {k} from frame {start}) reaches past the "
+                                 f"{n_frames} frames of the trajectory")
         return slice(start, start + t * k, k)
 
 
 class WindowPrefetcher:
     """Iterates device-resident feature dicts, one protein window per item: while the consumer trains on window i, a worker
-    thread slices window i+1 into pinned staging buffers and a side stream copies it to the device and featurises it."""
+    thread has a side stream copy window i+1 to the device and featurise it.
+
+    Each item's tensors are recorded on the stream that is current when the item is handed out, so their memory is not
+    reused before the work queued there on them has run, even when the consumer drops the item long before.  A consumer
+    that reads them on yet another stream must ``record_stream`` that stream itself.  Leaving the loop early (``break``)
+    stops the worker thread."""
 
     def __init__(self, store: TrajectoryStore, rows: Sequence[Tuple[str, str, str, str]], device, training: bool = True, depth: int = 2,
                  diffuser=None, min_t: float = 0.01, generator: Optional[torch.Generator] = None, targets: bool = False):
@@ -118,7 +137,8 @@ class WindowPrefetcher:
         docstring); ``min_t`` is the loader's ``data_conf.min_t``; ``generator`` (a CUDA generator on ``device``) feeds t
         and the diffusion draws, default: the device's default generator.  ``targets`` adds the evaluation targets
         ``atom37_pos`` [nf, N, 37, 3] and ``atom37_mask`` [nf, N, 37], fp64 as ``_process_csv_row`` returns them (:249-250),
-        which ``metrics.evaluate_window`` scores the sample against."""
+        which ``metrics.evaluate_window`` scores the sample against (atoms outside the mask keep the archive's coordinates,
+        which the loader zeroes; every metric masks them)."""
         dev = torch.device(device)
         if dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device())
@@ -130,35 +150,18 @@ class WindowPrefetcher:
         if diffuser is not None:
             diffuser.tables(self.device)                    # built once, before the side stream reads them
             self.stream.wait_stream(torch.cuda.current_stream(self.device))
-        self._staging: Dict = {}
-        self._slot: Dict[str, int] = {}
-        self._events: list = []
-
-    def _stage(self, name: str, src: torch.Tensor, sl: slice) -> torch.Tensor:
-        """The (possibly strided) frame window gathered into a pinned staging buffer: a ring of depth + 1 buffers per field,
-        so a buffer is reused only after the consumer has received the window that was copied from it."""
-        n = len(range(*sl.indices(src.shape[0])))
-        shape = (n,) + tuple(src.shape[1:])
-        ring = self._staging.setdefault((name, shape, src.dtype), [])
-        if len(ring) <= self.depth:
-            buf = torch.empty(shape, dtype=src.dtype)
-            ring.append(buf.pin_memory() if self.store.pin else buf)
-        slot = self._slot.get(name, 0)
-        self._slot[name] = (slot + 1) % (self.depth + 1)
-        buf = ring[min(slot, len(ring) - 1)]
-        buf.copy_(src[sl])
-        return buf
+        self._thread: Optional[threading.Thread] = None
 
     def _make(self, row) -> Tuple[Dict[str, torch.Tensor], torch.cuda.Event]:
         ent = self.store.protein(*row)
-        # the staging buffers of this window were last used depth + 1 windows ago: that copy must have left the host
-        if len(self._events) > self.depth:
-            self._events[-(self.depth + 1)].synchronize()
         sl = self.store.window_index(ent["atom37"].shape[0], self.training)
         nf = self.store.frame_time
         with torch.cuda.stream(self.stream):
             cp = lambda t: t.to(self.device, non_blocking=True)
-            atom37 = cp(self._stage("atom37", ent["atom37"], sl))
+            # the contiguous frame range straight from the store, whose pinned memory nothing writes; every step-th frame
+            # is then taken on the device
+            frames = lambda t: cp(t[sl.start:sl.stop])[::sl.step].contiguous()
+            atom37 = frames(ent["atom37"])
             atom_mask = cp(ent["atom_mask"])
             feats = featurize_window(atom37, atom_mask, cp(ent["aatype"]))
             if self.targets:
@@ -168,7 +171,7 @@ class WindowPrefetcher:
                 "aatype": cp(ent["aatype"]).unsqueeze(0).expand(nf, -1),
                 "seq_idx": cp(ent["residue_index"]).unsqueeze(0).expand(nf, -1),
                 "residue_index": cp(ent["residue_index"]).unsqueeze(0).expand(nf, -1),
-                "force": cp(self._stage("force", ent["force"], sl)), "vel": cp(self._stage("vel", ent["vel"], sl)),
+                "force": frames(ent["force"]), "vel": frames(ent["vel"]),
                 "node_repr": cp(ent["node_repr"]), "edge_repr": cp(ent["edge_repr"]),
                 "fixed_mask": torch.zeros(nf, atom37.shape[1], dtype=torch.float64, device=self.device),
                 "sc_ca_t": torch.zeros(nf, atom37.shape[1], 3, dtype=torch.float32, device=self.device),
@@ -177,8 +180,6 @@ class WindowPrefetcher:
                 feats.update(self._noise(feats["rigids_0"]))
             ev = torch.cuda.Event()
             ev.record(self.stream)
-        self._events.append(ev)
-        del self._events[:-(self.depth + 2)]
         return feats, ev
 
     def _noise(self, rigids_0: torch.Tensor) -> Dict[str, torch.Tensor]:
@@ -198,23 +199,41 @@ class WindowPrefetcher:
     def __iter__(self) -> Iterator[Dict[str, torch.Tensor]]:
         import queue
         q: "queue.Queue" = queue.Queue(maxsize=self.depth)
+        stop = threading.Event()
+
+        def put(item) -> bool:
+            """Queue ``item`` unless the consumer has left; False once it has."""
+            while not stop.is_set():
+                try:
+                    q.put(item, timeout=0.05)
+                    return True
+                except queue.Full:
+                    pass
+            return False
 
         def work():
             try:
                 torch.cuda.set_device(self.device)
                 for row in self.rows:
-                    q.put(self._make(row))
-                q.put(None)
+                    if not put(self._make(row)):
+                        return
+                put(None)
             except BaseException as e:       # noqa: BLE001  (hand the failure to the consumer instead of blocking it forever)
-                q.put(e)
-        th = threading.Thread(target=work, daemon=True)
-        th.start()
-        while True:
-            item = q.get(timeout=600)
-            if item is None:
-                break
-            if isinstance(item, BaseException):
-                raise RuntimeError("WindowPrefetcher worker failed") from item
-            feats, ev = item
-            torch.cuda.current_stream(self.device).wait_event(ev)
-            yield feats
+                put(e)
+        self._thread = threading.Thread(target=work, daemon=True)
+        self._thread.start()
+        try:
+            while True:
+                item = q.get(timeout=600)
+                if item is None:
+                    break
+                if isinstance(item, BaseException):
+                    raise RuntimeError("WindowPrefetcher worker failed") from item
+                feats, ev = item
+                consumer = torch.cuda.current_stream(self.device)
+                consumer.wait_event(ev)
+                for v in feats.values():
+                    v.record_stream(consumer)
+                yield feats
+        finally:
+            stop.set()

@@ -225,31 +225,70 @@ def run_loss():
     torch.save(res, os.path.join(OUT, "loss.pt"))
 
 
-def run_loader():
-    """tests/golden/loader.pt: what the UNMODIFIED loader computes for one window of a synthetic trajectory written in the
-    reference's on-disk formats: PdbDataset._process_csv_row (src/data/Dfold_data_loader_dynamic.py:192-259) and the
-    rigids_0 lines of __getitem__ (:323-330), training-mode window selection with numpy seed 5."""
-    import tempfile
+def _loader_row(row, training, **data_conf):
+    """PdbDataset._process_csv_row of the UNMODIFIED loader (src/data/Dfold_data_loader_dynamic.py:192-259) on one csv row."""
     from types import SimpleNamespace
-    import numpy as np
-    from oracle import synth_traj
     ref_shims.install_trainer_stubs()
     from src.data import Dfold_data_loader_dynamic as L
+    ds = object.__new__(L.PdbDataset)
+    ds._is_training = training
+    ds._data_conf = SimpleNamespace(**data_conf)
+    return ds._process_csv_row(row[0], row[1], row[2], None)
+
+
+def _loader_fixture(feats, extra=()):
+    """The loader fields the tests compare, plus the rigids_0 lines of __getitem__ (:323-330)."""
+    rig = RefRU.Rigid.from_tensor_4x4(feats["rigidgroups_0"])[:, :, 0]
+    res = {k: feats[k].clone() for k in ("aatype", "seq_idx", "res_mask", "torsion_angles_sin_cos", "alt_torsion_angles_sin_cos",
+                                         "torsion_angles_mask", "force", "vel") + tuple(extra)}
+    res["rigids_0"] = rig.to_tensor_7()
+    res["rot_0"] = rig.get_rots().get_rot_mats()
+    return res
+
+
+def run_loader():
+    """tests/golden/loader.pt: what the UNMODIFIED loader computes for one window of a synthetic trajectory written in the
+    reference's on-disk formats: PdbDataset._process_csv_row and the rigids_0 lines of __getitem__, training-mode window
+    selection with numpy seed 5."""
+    import tempfile
+    import numpy as np
+    from oracle import synth_traj
     traj = synth_traj.make_trajectory()
     with tempfile.TemporaryDirectory() as d:
         row = synth_traj.write_files(traj, d)
-        ds = object.__new__(L.PdbDataset)
-        ds._is_training = True
-        ds._data_conf = SimpleNamespace(frame_time=3, keep_first=8, frame_sample_step=2, fix_sample_start=0)
         np.random.seed(5)
-        feats = ds._process_csv_row(row[0], row[1], row[2], None)
-    rig = RefRU.Rigid.from_tensor_4x4(feats["rigidgroups_0"])[:, :, 0]
-    res = {k: feats[k].clone() for k in ("aatype", "seq_idx", "res_mask", "torsion_angles_sin_cos", "alt_torsion_angles_sin_cos",
-                                         "torsion_angles_mask", "force", "vel")}
-    res["rigids_0"] = rig.to_tensor_7()
-    res["rot_0"] = rig.get_rots().get_rot_mats()
+        feats = _loader_row(row, True, frame_time=3, keep_first=8, frame_sample_step=2, fix_sample_start=0)
+    res = _loader_fixture(feats)
     torch.save(res, os.path.join(OUT, "loader.pt"))
     print("[golden] loader:", {k: tuple(v.shape) for k, v in res.items()})
+
+
+LOADER_EVAL = dict(T=12, frame_time=3, keep_first=8, frame_sample_step=2, fix_sample_start=4, fix_sample_start_error=10)
+
+
+def run_loader_eval():
+    """tests/golden/loader_eval.pt: the evaluation window of the UNMODIFIED loader on a 12-frame synthetic trajectory with
+    keep_first=8, fix_sample_start=4, frame_time=3, frame_sample_step=2.  Evaluation ignores keep_first (:214-218), so the
+    window is frames 4, 6 and 8, past the first 8.  Also the ValueError message select_first_samples raises (:178-190) when
+    fix_sample_start=10 leaves fewer than frame_time frames."""
+    import tempfile
+    from oracle import synth_traj
+    c = LOADER_EVAL
+    conf = dict(frame_time=c["frame_time"], keep_first=c["keep_first"], frame_sample_step=c["frame_sample_step"])
+    with tempfile.TemporaryDirectory() as d:
+        row = synth_traj.write_files(synth_traj.make_trajectory(T=c["T"]), d)
+        feats = _loader_row(row, False, fix_sample_start=c["fix_sample_start"], **conf)
+        try:
+            _loader_row(row, False, fix_sample_start=c["fix_sample_start_error"], **conf)
+        except ValueError as e:
+            err = str(e)
+        else:
+            raise AssertionError("the reference loader accepted a window past the trajectory")
+    res = _loader_fixture(feats, extra=("atom37_pos", "atom37_mask"))
+    res["case"] = dict(c)
+    res["error"] = err
+    torch.save(res, os.path.join(OUT, "loader_eval.pt"))
+    print("[golden] loader_eval:", {k: tuple(v.shape) for k, v in res.items() if torch.is_tensor(v)}, "error:", err)
 
 
 def boundary_batch():
@@ -298,6 +337,7 @@ if __name__ == "__main__":
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "loader":
         run_loader()
+        run_loader_eval()
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "loss":
         run_loss()
@@ -311,6 +351,7 @@ if __name__ == "__main__":
     run_reverse()
     run_loss()
     run_loader()
+    run_loader_eval()
     run_transitions()
     for n, c in NET_CASES.items():
         run_net(n, c)
