@@ -21,6 +21,10 @@ comparable to the device time, so the step is:
   computes the step's lr from the device step counter, and Adam reads it from device memory (``current_lr``);
 * ``accumulate=k`` averages the gradient over k windows per rank before the update (k input slots, filled with
   ``load(feats, slot=i)``): one optimizer step then sees the mean over world_size * k windows, as DDP over that many ranks;
+* ``loss_reads_window=True`` calls ``loss_fn(out, slot)`` with the static input dict of the window the output came from,
+  so an objective that needs its window's targets (``loss.score_network_loss``) reads slot i's in capture and in every
+  replay; a loss function that returns ``(loss, aux_data)`` has slot 0's ``aux_data`` kept in static device tensors,
+  ``aux``, overwritten by every step and never read back to the host;
 * ``state_dict()`` / ``load_state_dict()`` save and resume the weights and the Adam(amsgrad) state in the reference
   trainer's checkpoint format, loading in place so the captured graph keeps running (checkpoint.py).
 """
@@ -87,7 +91,7 @@ class TrainStep:
     def __init__(self, net: torch.nn.Module, loss_fn: Callable[[Dict[str, torch.Tensor]], torch.Tensor],
                  example_feats: Dict[str, torch.Tensor], *, lr: float = 1e-4, world_size: int = 1, graph: bool = True,
                  warmup: int = 3, max_grad_norm: Optional[float] = None, lr_schedule: Optional[AlphaFoldSchedule] = None,
-                 accumulate: int = 1):
+                 accumulate: int = 1, loss_reads_window: bool = False):
         self.max_grad_norm = _check_max_grad_norm(max_grad_norm)
         if lr_schedule is not None and not isinstance(lr_schedule, AlphaFoldSchedule):
             raise ValueError(f"lr_schedule must be None or an AlphaFoldSchedule, got {type(lr_schedule).__name__}")
@@ -102,6 +106,7 @@ class TrainStep:
                              f"DFOLD_ALLREDUCE_CHUNKS={self.chunks} updates each piece as soon as it is reduced: "
                              "unset it to clip")
         self.net, self.loss_fn, self.world = net, loss_fn, world_size
+        self.loss_reads_window = bool(loss_reads_window)
         # the summed gradient of world_size ranks x accumulate windows becomes their mean
         self.grad_scale = 1.0 / (world_size * self.accumulate)
         self.params = [p for p in net.parameters() if p.requires_grad]
@@ -145,6 +150,8 @@ class TrainStep:
         self.slots = [{k: v.clone() for k, v in example_feats.items()} for _ in range(self.accumulate)]
         self.static = self.slots[0]
         self.loss = torch.zeros((), dtype=torch.float32, device=dev)
+        # slot 0's aux_data when loss_fn returns (loss, aux_data): allocated by the first (warm-up) step, then overwritten in place
+        self.aux: Optional[Dict[str, torch.Tensor]] = None
         # the global norm of the mean gradient before clipping, overwritten by every step (None: no clipping, no norm)
         self.grad_norm: Optional[torch.Tensor] = None
         if self.max_grad_norm is not None:
@@ -212,6 +219,8 @@ class TrainStep:
             self.flat_grad.zero_()
             if self.grad_norm is not None:
                 self.grad_norm.zero_()
+            for v in (self.aux or {}).values():
+                v.zero_()
             if self.current_lr is not None:
                 self.current_lr.fill_(self.schedule.lr(0))
         _kernels.invalidate_weight_cache()
@@ -221,7 +230,12 @@ class TrainStep:
         self.flat_grad.zero_()
         for i, feats in enumerate(self.slots):
             out = self.net(dict(feats))
-            loss = self.loss_fn(out)
+            loss = self.loss_fn(out, feats) if self.loss_reads_window else self.loss_fn(out)
+            if isinstance(loss, tuple):
+                loss, aux = loss
+                if i == 0:
+                    self._keep_aux(aux)
+                del aux
             del out                                  # with the backward below, frees the window's activations before the next
             prev, _kernels.GRAD_ACCUMULATE_INPLACE = _kernels.GRAD_ACCUMULATE_INPLACE, True     # wgrad kernels add into the flat buffer
             try:
@@ -256,6 +270,13 @@ class TrainStep:
             if self.opt is not None and self.grad_scale != 1.0:
                 self.flat_grad.mul_(self.grad_scale)        # (the fused optimizer scales the summed gradient on the fly)
             self.optimizer_step()
+
+    def _keep_aux(self, aux: Dict[str, torch.Tensor]):
+        if self.aux is None:
+            self.aux = {k: v.detach().clone() for k, v in aux.items()}
+        else:
+            for k, v in aux.items():
+                self.aux[k].copy_(v.detach())
 
     def _schedule_lr(self, step: torch.Tensor):
         """current_lr = the schedule's lr at `step` optimizer steps taken (device counter, read before this step's tick)."""
