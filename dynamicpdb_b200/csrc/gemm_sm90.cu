@@ -507,8 +507,9 @@ void default_batching(GemmParams& p) {
 
 
 // Tile width: every CTA owns one SM (up to 227 KB of shared memory; the 128-wide ring takes 192 KB), so the launch runs
-// in ceil(tiles / SMs) waves whose duration is proportional to BN.  Pick the width with the smallest waves x BN
-// (ties -> the wider tile, which re-reads the A operand less).  `row_tiles` = 128-row tiles x batches / taps in the other
+// in ceil(tiles / SMs) waves, here taken to last in proportion to BN.  Pick the width with the smallest waves x BN
+// (ties -> the wider tile, which re-reads the A operand less).  A 64-wide tile in fact takes ~0.6 of a 128-wide one's
+// time, so the convolutions choose their width from that measured cost through the *_bn entry points (DESIGN.md §4).  `row_tiles` = 128-row tiles x batches / taps in the other
 // grid dimensions.  BN stops at 128: a 64 x BN wgmma tile per consumer warpgroup holds BN / 2 accumulator registers per
 // thread twice over (tensor-core partial sum + promoted sum), and BN = 256 would need 256 of them.
 int pick_bn(long n_out, long row_tiles) {
@@ -534,16 +535,18 @@ extern "C" int dfold_debug_gemm_stats(long long* buf) {
     return 0;
 }
 
-extern "C" int dfold_gemm_bf16x3(
-    const uint16_t* a_hi, const uint16_t* a_lo, long F, long F_out, int f_start, long Nr, long K, long lda,
-    const uint16_t* b_hi, const uint16_t* b_lo, long n_out, long ldb, int taps_f, int taps_n,
-    float* out, long ldo, const float* bias, const float* residual, long ldr,
-    float alpha, float beta, int act, void* stream) {
-    DFOLD_REQUIRE(F > 0 && F_out > 0 && Nr > 0 && K > 0 && n_out > 0, "dfold_gemm_bf16x3: empty problem");
-    DFOLD_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "dfold_gemm_bf16x3: lda/ldb must be multiples of 8 (got %ld, %ld)", lda, ldb);
-    DFOLD_REQUIRE(taps_f >= 1 && taps_n >= 1 && (taps_f & 1) && (taps_n & 1), "dfold_gemm_bf16x3: tap grid must be odd");
-    const long row_tiles = F_out * cdiv(Nr, BM);
-    const int bn = pick_bn(n_out, row_tiles);
+namespace dfold {
+namespace {
+
+// dfold_gemm_bf16x3 on tiles `bn` wide.  `name`: the calling entry point, for error messages.
+int gemm_kmajor(const char* name, const uint16_t* a_hi, const uint16_t* a_lo, long F, long F_out, int f_start, long Nr,
+                long K, long lda, const uint16_t* b_hi, const uint16_t* b_lo, long n_out, long ldb, int taps_f, int taps_n,
+                float* out, long ldo, const float* bias, const float* residual, long ldr,
+                float alpha, float beta, int act, int bn, void* stream) {
+    DFOLD_REQUIRE(F > 0 && F_out > 0 && Nr > 0 && K > 0 && n_out > 0, "%s: empty problem", name);
+    DFOLD_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "%s: lda/ldb must be multiples of 8 (got %ld, %ld)", name, lda, ldb);
+    DFOLD_REQUIRE(taps_f >= 1 && taps_n >= 1 && (taps_f & 1) && (taps_n & 1), "%s: tap grid must be odd", name);
+    DFOLD_REQUIRE(bn == 64 || bn == 128, "%s: tile width must be 64 or 128 (got %d)", name, bn);
     CUtensorMap maps[4];
     // A: dims (K, Nr, F)   B: dims (K, n_out, taps)
     if (make_map(&maps[0], a_hi, K, Nr, F, lda, Nr * lda, BK, BM, 1)) return 1;
@@ -567,26 +570,20 @@ extern "C" int dfold_gemm_bf16x3(
     p.f_start = f_start;
     cudaStream_t st = as_stream(stream);
     // Every output element is produced by one CTA in a fixed k order (no split-K with atomics): the result is the same
-    // from run to run.
+    // from run to run, and the same at either tile width.
     dim3 grid((unsigned)cdiv(n_out, bn), (unsigned)(F_out * p.tiles_per_frame), 1);
-    int rc;
-    if (bn == 128) rc = launch<128>(maps, p, grid, st);
-    else rc = launch<64>(maps, p, grid, st);
-    return rc;
+    if (bn == 128) return launch<128>(maps, p, grid, st);
+    return launch<64>(maps, p, grid, st);
 }
 
-// out[tap][m][n] = alpha * sum_{f, j} A[f][j][m] * B[f + df(tap)][j + dn(tap)][n]      (weight gradient; K = pixels)
-// A planes [F][Nr][lda] (e.g. the gated output gradient, m = output channel), B planes [Fb][Nr][ldb] (the layer input,
-// n = input channel, frame f of A pairs with frame f + b_f_add of B: cropped convolutions): the SAME pixel-major
-// planes the forward / data-gradient GEMMs use, read MN-major.
-extern "C" int dfold_gemm_wgrad_bf16x3(
-    const uint16_t* a_hi, const uint16_t* a_lo, long M, long lda,
-    const uint16_t* b_hi, const uint16_t* b_lo, long Nn, long ldb,
-    long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
-    float* out, long ldo, float alpha, void* stream) {
-    DFOLD_REQUIRE(M > 0 && Nn > 0 && F > 0 && Fb > 0 && Nr > 0, "dfold_gemm_wgrad_bf16x3: empty problem");
-    DFOLD_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "dfold_gemm_wgrad_bf16x3: lda/ldb must be multiples of 8 (got %ld, %ld)", lda, ldb);
-    const int bn = pick_bn(Nn, cdiv(M, BM) * taps_f * taps_n);
+// dfold_gemm_wgrad_bf16x3 on tiles `bn` wide.
+int gemm_wgrad(const char* name, const uint16_t* a_hi, const uint16_t* a_lo, long M, long lda,
+               const uint16_t* b_hi, const uint16_t* b_lo, long Nn, long ldb,
+               long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
+               float* out, long ldo, float alpha, int bn, void* stream) {
+    DFOLD_REQUIRE(M > 0 && Nn > 0 && F > 0 && Fb > 0 && Nr > 0, "%s: empty problem", name);
+    DFOLD_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "%s: lda/ldb must be multiples of 8 (got %ld, %ld)", name, lda, ldb);
+    DFOLD_REQUIRE(bn == 64 || bn == 128, "%s: tile width must be 64 or 128 (got %d)", name, bn);
     CUtensorMap maps[4];
     // dims (channel, residue, frame); boxes of 64 channels x 64 residues
     if (make_map(&maps[0], a_hi, M, Nr, F, lda, Nr * lda, 64, BK, 1)) return 1;
@@ -609,6 +606,51 @@ extern "C" int dfold_gemm_wgrad_bf16x3(
     cudaStream_t st = as_stream(stream);
     if (bn == 128) return launch<128>(maps, p, grid, st);
     return launch<64>(maps, p, grid, st);
+}
+
+}  // namespace
+}  // namespace dfold
+
+extern "C" int dfold_gemm_bf16x3(
+    const uint16_t* a_hi, const uint16_t* a_lo, long F, long F_out, int f_start, long Nr, long K, long lda,
+    const uint16_t* b_hi, const uint16_t* b_lo, long n_out, long ldb, int taps_f, int taps_n,
+    float* out, long ldo, const float* bias, const float* residual, long ldr,
+    float alpha, float beta, int act, void* stream) {
+    return gemm_kmajor("dfold_gemm_bf16x3", a_hi, a_lo, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f,
+                       taps_n, out, ldo, bias, residual, ldr, alpha, beta, act, pick_bn(n_out, F_out * cdiv(Nr, BM)), stream);
+}
+
+// dfold_gemm_bf16x3 on tiles `bn` (64 or 128) wide, for callers that weigh the widths themselves.
+extern "C" int dfold_gemm_bf16x3_bn(
+    const uint16_t* a_hi, const uint16_t* a_lo, long F, long F_out, int f_start, long Nr, long K, long lda,
+    const uint16_t* b_hi, const uint16_t* b_lo, long n_out, long ldb, int taps_f, int taps_n,
+    float* out, long ldo, const float* bias, const float* residual, long ldr,
+    float alpha, float beta, int act, int bn, void* stream) {
+    return gemm_kmajor("dfold_gemm_bf16x3_bn", a_hi, a_lo, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f,
+                       taps_n, out, ldo, bias, residual, ldr, alpha, beta, act, bn, stream);
+}
+
+// out[tap][m][n] = alpha * sum_{f, j} A[f][j][m] * B[f + df(tap)][j + dn(tap)][n]      (weight gradient; K = pixels)
+// A planes [F][Nr][lda] (e.g. the gated output gradient, m = output channel), B planes [Fb][Nr][ldb] (the layer input,
+// n = input channel, frame f of A pairs with frame f + b_f_add of B: cropped convolutions): the SAME pixel-major
+// planes the forward / data-gradient GEMMs use, read MN-major.
+extern "C" int dfold_gemm_wgrad_bf16x3(
+    const uint16_t* a_hi, const uint16_t* a_lo, long M, long lda,
+    const uint16_t* b_hi, const uint16_t* b_lo, long Nn, long ldb,
+    long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
+    float* out, long ldo, float alpha, void* stream) {
+    return gemm_wgrad("dfold_gemm_wgrad_bf16x3", a_hi, a_lo, M, lda, b_hi, b_lo, Nn, ldb, F, Fb, b_f_add, Nr, taps_f, taps_n,
+                      out, ldo, alpha, pick_bn(Nn, cdiv(M, BM) * taps_f * taps_n), stream);
+}
+
+// dfold_gemm_wgrad_bf16x3 on tiles `bn` (64 or 128) wide.
+extern "C" int dfold_gemm_wgrad_bf16x3_bn(
+    const uint16_t* a_hi, const uint16_t* a_lo, long M, long lda,
+    const uint16_t* b_hi, const uint16_t* b_lo, long Nn, long ldb,
+    long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
+    float* out, long ldo, float alpha, int bn, void* stream) {
+    return gemm_wgrad("dfold_gemm_wgrad_bf16x3_bn", a_hi, a_lo, M, lda, b_hi, b_lo, Nn, ldb, F, Fb, b_f_add, Nr, taps_f,
+                      taps_n, out, ldo, alpha, bn, stream);
 }
 
 // Batched K-major GEMM (no taps): for every row tile of "frame" b in [0, n_batches), hb = b % bmod:

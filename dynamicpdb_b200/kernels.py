@@ -46,7 +46,9 @@ _SIGS = {
     "dfold_compose_q_update_fwd": "pppppplp",
     "dfold_compose_q_update_bwd": "pppppppplp",
     "dfold_gemm_bf16x3": "pplli" + "lll" + "ppllii" + "pl" + "p" + "pl" + "ffi" + "p",
+    "dfold_gemm_bf16x3_bn": "pplli" + "lll" + "ppllii" + "pl" + "p" + "pl" + "ffi" + "i" + "p",
     "dfold_gemm_wgrad_bf16x3": "ppll" + "ppll" + "llilii" + "plf" + "p",
+    "dfold_gemm_wgrad_bf16x3_bn": "ppll" + "ppll" + "llilii" + "plf" + "i" + "p",
     "dfold_ipa_attn_fwd": "plplppplpppp" + "iiiiiiii" + "ff" + "ppp",
     "dfold_ipa_attn_bwd": "plplppplpppp" + "iiiiiiii" + "ff" + "ppp" + "ppppppppp" + "p",
     "dfold_ipa_pre_bwd": "pp" + "iiiiiii" + "pp" + "pppp" + "p",
@@ -355,18 +357,46 @@ def _conv_planes(w: torch.Tensor):
     return _cache_get("conv", w, build)
 
 
+# Time of one 128 x BN output tile of the split-bf16 GEMM per k-block, relative to a 128-wide one.  Over the 30
+# convolution GEMMs of a training step a 64-wide tile costs 0.58-0.75 of a 128-wide one, median 0.61 in each of two runs
+# (tests/devtools/dev_gemm_width.py, H100 80GB HBM3 at a 700 W power limit; DESIGN.md §4, "Tile width"): half the work
+# for 0.6 of the time.  Any value in (10/19, 2/3) makes the same choices at that step's wave counts.
+TILE_COST = {64: 0.6, 128: 1.0}
+
+
+def _conv_bn(n_out: int, row_tiles: int, dev) -> int:
+    """Tile width of a convolution GEMM with `n_out` output columns and `row_tiles` 128-row tiles (times taps): the launch
+    runs in ceil(tiles / SMs) waves of one tile per SM, so pick the width with the least waves x TILE_COST (ties -> 128)."""
+    sms = _sm_count(dev)
+
+    def cost(bn):
+        tiles = -(-n_out // bn) * row_tiles
+        return -(-tiles // sms) * TILE_COST[bn]
+    return 64 if cost(64) < cost(128) else 128
+
+
 def _gemm(a_hi, a_lo, F, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f, taps_n, out, ldo, bias, residual, ldr, alpha, beta, act,
-          F_out=None, f_start=0):
+          F_out=None, f_start=0, bn=None):
+    """dfold_gemm_bf16x3, or with ``bn`` set its explicit-width form dfold_gemm_bf16x3_bn."""
     F_out = F if F_out is None else F_out
+    args = (a_hi, a_lo, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f, taps_n, out, ldo, bias, residual, ldr,
+            alpha, beta, act)
     with _timed("gemm_bf16x3", 2.0 * F_out * Nr * K * n_out * taps_f * taps_n, f"kmajor F{F_out} N{Nr} K{K} out{n_out} taps{taps_f * taps_n}"):
-        launch("dfold_gemm_bf16x3", a_hi, a_lo, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f, taps_n,
-               out, ldo, bias, residual, ldr, alpha, beta, act)
+        if bn is None:
+            launch("dfold_gemm_bf16x3", *args)
+        else:
+            launch("dfold_gemm_bf16x3_bn", *args, bn)
 
 
-def _gemm_wgrad(a, M, lda, b, Nn, ldb, F, Nr, taps_f, taps_n, out, ldo, Fb=None, b_f_add=0):
+def _gemm_wgrad(a, M, lda, b, Nn, ldb, F, Nr, taps_f, taps_n, out, ldo, Fb=None, b_f_add=0, bn=None):
+    """dfold_gemm_wgrad_bf16x3, or with ``bn`` set dfold_gemm_wgrad_bf16x3_bn."""
     Fb = F if Fb is None else Fb
+    args = (a[0], a[1], M, lda, b[0], b[1], Nn, ldb, F, Fb, b_f_add, Nr, taps_f, taps_n, out, ldo, 1.0)
     with _timed("gemm_bf16x3", 2.0 * F * Nr * M * Nn * taps_f * taps_n, f"wgrad F{F} N{Nr} M{M} n{Nn} taps{taps_f * taps_n}"):
-        launch("dfold_gemm_wgrad_bf16x3", a[0], a[1], M, lda, b[0], b[1], Nn, ldb, F, Fb, b_f_add, Nr, taps_f, taps_n, out, ldo, 1.0)
+        if bn is None:
+            launch("dfold_gemm_wgrad_bf16x3", *args)
+        else:
+            launch("dfold_gemm_wgrad_bf16x3_bn", *args, bn)
 
 
 _ACT = {None: 0, "relu": 1}
@@ -490,7 +520,7 @@ class _Conv5x5Fn(Function):
         (a_hi, a_lo), _ = _split2d(x2)
         f_hi, f_lo, _, _ = _conv_planes(w)
         _gemm(a_hi, a_lo, F_, N_, Ci, Ci, f_hi, f_lo, Co, f_hi.shape[2], kh, kw, out, Co, _f32c(b) if b is not None else None,
-              r2, Co, 1.0, 1.0, 1 if relu else 0, F_out=Fo, f_start=crop)
+              r2, Co, 1.0, 1.0, 1 if relu else 0, F_out=Fo, f_start=crop, bn=_conv_bn(Co, Fo * -(-N_ // 128), x.device))
         ctx.save_for_backward(a_hi, a_lo, w, out if relu else None, r2 if relu else None)
         ctx.meta = (x.shape, relu, b is not None, residual is not None, crop)
         ctx.w_param = w if isinstance(w, torch.nn.Parameter) else None
@@ -526,7 +556,7 @@ class _Conv5x5Fn(Function):
             _, _, d_hi, d_lo = _conv_planes(w)
             dx = torch.empty((F_ * N_, Ci), dtype=torch.float32, device=g.device)
             _gemm(g_hi, g_lo, Fo, N_, Co, Co, d_hi, d_lo, Ci, d_hi.shape[2], kh, kw, dx, Ci, None, None, 0, 1.0, 0.0, 0,
-                  F_out=F_, f_start=-crop)
+                  F_out=F_, f_start=-crop, bn=_conv_bn(Ci, F_ * -(-N_ // 128), g.device))
             dx = dx.reshape(F_, N_, Ci)
         if acc is not None and not side:
             wgrad(acc, 1)
@@ -540,7 +570,8 @@ def _conv_wgrad(g_hi, g_lo, x_hi, x_lo, Co, Ci, kh, kw, F_, Fo, N_, crop, out, a
     """Weight gradient of the convolution: the per-tap GEMMs into a [taps, Co, Ci] scratch (allocated on the current
     stream), then added into (add=1) or written to (add=0) ``out`` [Co, Ci, kh, kw]."""
     taps = torch.empty((kh * kw, Co, Ci), dtype=torch.float32, device=out.device)
-    _gemm_wgrad((g_hi, g_lo), Co, Co, (x_hi, x_lo), Ci, Ci, Fo, N_, kh, kw, taps, Ci, Fb=F_, b_f_add=crop)
+    _gemm_wgrad((g_hi, g_lo), Co, Co, (x_hi, x_lo), Ci, Ci, Fo, N_, kh, kw, taps, Ci, Fb=F_, b_f_add=crop,
+                bn=_conv_bn(Ci, -(-Co // 128) * kh * kw, out.device))
     launch("dfold_taps_to_param", taps, Co, Ci, kh * kw, out, add)
 
 

@@ -77,6 +77,13 @@ int dfold_gemm_bf16x3(const uint16_t* a_hi, const uint16_t* a_lo, long F, long F
                       float* out, long ldo, const float* bias, const float* residual, long ldr,
                       float alpha, float beta, int act, void* stream);
 
+/* dfold_gemm_bf16x3 on output tiles bn = 64 or 128 columns wide (dfold_gemm_bf16x3 picks the width itself).  Any other
+ * width is rejected.  Each output element is the same one-CTA, fixed-order k loop at either width. */
+int dfold_gemm_bf16x3_bn(const uint16_t* a_hi, const uint16_t* a_lo, long F, long F_out, int f_start, long Nr, long K,
+                         long lda, const uint16_t* b_hi, const uint16_t* b_lo, long n_out, long ldb, int taps_f, int taps_n,
+                         float* out, long ldo, const float* bias, const float* residual, long ldr,
+                         float alpha, float beta, int act, int bn, void* stream);
+
 /* Weight gradient: out[t][m][n] = alpha * sum_{f,j} A[f][j][m] * B[f + b_f_add + tf - taps_f/2][j + tn - taps_n/2][n]
  * A planes [F][Nr][lda] (gated output gradient, m = output channel), B planes [Fb][Nr][ldb] (layer input,
  * n = input channel) — the same pixel-major planes as above, consumed MN-major by the tensor core; out [taps][M][ldo]. */
@@ -84,6 +91,12 @@ int dfold_gemm_wgrad_bf16x3(const uint16_t* a_hi, const uint16_t* a_lo, long M, 
                             const uint16_t* b_hi, const uint16_t* b_lo, long Nn, long ldb,
                             long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
                             float* out, long ldo, float alpha, void* stream);
+
+/* dfold_gemm_wgrad_bf16x3 on output tiles bn = 64 or 128 columns wide; any other width is rejected. */
+int dfold_gemm_wgrad_bf16x3_bn(const uint16_t* a_hi, const uint16_t* a_lo, long M, long lda,
+                               const uint16_t* b_hi, const uint16_t* b_lo, long Nn, long ldb,
+                               long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
+                               float* out, long ldo, float alpha, int bn, void* stream);
 
 /* Batched K-major GEMM (no taps).  For every row tile of "frame" b in [0, n_batches), hb = b % bmod:
  *   out[(b / o_f_div) * Nr + n, hb * o_col_bstride + c] =
