@@ -83,13 +83,10 @@ def _names(keys, limit=4):
     return ", ".join(map(str, keys[:limit])) + (f" and {len(keys) - limit} more" if len(keys) > limit else "")
 
 
-def check_state(sd: dict, layout: FlatLayout, model_shapes: Dict[str, torch.Size], lr: float, schedule=None
-                ) -> Tuple[Dict[str, torch.Tensor], Optional[Dict[int, dict]], float]:
-    """Validates a checkpoint dict against the step it is to be loaded into and returns (model tensors by the network's
-    own names, optimizer state entries by parameter index or None for a weights-only load, the common step).  Raises
-    ValueError, naming the problem, for anything that would resume a different optimisation than the one saved.
-    ``schedule`` (train_step.AlphaFoldSchedule or None): the checkpoint's lr must be ``schedule.lr(step)``, the lr a
-    scheduler stepped once per optimizer step leaves in the param group, instead of ``lr``."""
+def check_model(sd: dict, model_shapes: Dict[str, torch.Size]) -> Dict[str, torch.Tensor]:
+    """Validates the ``model`` state_dict of a checkpoint dict against a network's ``{name: shape}`` and returns its
+    tensors by the network's own names (``module.`` stripped).  Raises ValueError naming the unknown or missing keys, or
+    the first tensor whose shape differs, so that a strict ``load_state_dict`` of the result cannot fail half-way."""
     if not isinstance(sd, dict) or not isinstance(sd.get("model"), dict):
         raise ValueError("checkpoint has no 'model' state_dict")
     model = strip_module_prefix(sd["model"])
@@ -101,6 +98,17 @@ def check_state(sd: dict, layout: FlatLayout, model_shapes: Dict[str, torch.Size
         if not torch.is_tensor(model[k]) or tuple(model[k].shape) != tuple(shape):
             got = tuple(model[k].shape) if torch.is_tensor(model[k]) else type(model[k]).__name__
             raise ValueError(f"checkpoint model '{k}' has shape {got}, the network {tuple(shape)}")
+    return model
+
+
+def check_state(sd: dict, layout: FlatLayout, model_shapes: Dict[str, torch.Size], lr: float, schedule=None
+                ) -> Tuple[Dict[str, torch.Tensor], Optional[Dict[int, dict]], float]:
+    """Validates a checkpoint dict against the step it is to be loaded into and returns (model tensors by the network's
+    own names, optimizer state entries by parameter index or None for a weights-only load, the common step).  Raises
+    ValueError, naming the problem, for anything that would resume a different optimisation than the one saved.
+    ``schedule`` (train_step.AlphaFoldSchedule or None): the checkpoint's lr must be ``schedule.lr(step)``, the lr a
+    scheduler stepped once per optimizer step leaves in the param group, instead of ``lr``."""
+    model = check_model(sd, model_shapes)
     opt = sd.get("optimizer")
     if opt is None:
         return model, None, 0.0

@@ -10,6 +10,8 @@ cannot keep one GPU fed, let alone eight.  Here:
 * ``TrajectoryStore`` keeps each protein's trajectory decoded ONCE, in pinned host memory (atom37 coordinates as fp32:
   that is what the archive holds), and hands out frame windows with the reference's own index arithmetic and random
   stream (``select_random_samples`` / ``select_first_samples``, :164-190);
+* ``EvaluationStore`` is the store of an evaluation over a test split: it pins only each window's frames and keeps
+  nothing once the window is built;
 * ``featurize_window`` computes ``rigids_0`` and the torsion features of a window with one kernel on the device
   (csrc/featurize.cu), from the fp32 coordinates of the ``frame_time`` selected frames only;
 * ``WindowPrefetcher`` overlaps the next window's host->device copy (side stream, straight from the store's pinned
@@ -76,29 +78,25 @@ class TrajectoryStore:
         starts at ``fix_sample_start`` whatever ``keep_first`` is (:214-218)."""
         if atlas_npz in self._cache:
             return self._cache[atlas_npz]
-        with np.load(atlas_npz, allow_pickle=True) as zf:
-            z = {k: zf[k] for k in ("all_atom_positions", "all_atom_mask", "aatype", "residue_index")}
-        with open(force_path.replace(".pkl", "_Ca.pkl"), "rb") as f:
-            force = pickle.load(f)
-        with open(vel_path.replace(".pkl", "_ca.pkl"), "rb") as f:
-            vel = pickle.load(f)
-        with np.load(embed_path) as ef:
-            emb = {k: ef[k] for k in ("node_repr", "edge_repr")}
         kf = self.keep_first
         if kf is not None:
             kf = max(kf, self.fix_start + self.frame_time * self.step)
-        ent = {
-            "atom37": self._pin(z["all_atom_positions"][:kf], torch.float32),                 # [T,N,37,3]
-            "force": self._pin(np.asarray(force)[:kf], torch.float64),                        # [T,N,3] (the loader's dtype)
-            "vel": self._pin(np.asarray(vel)[:kf], torch.float64),
-            "atom_mask": self._pin(z["all_atom_mask"], torch.float32),                        # [N,37]
-            "aatype": torch.from_numpy(np.argmax(z["aatype"], axis=-1)).long(),               # [N]
-            "residue_index": torch.from_numpy(np.asarray(z["residue_index"])).long(),
-            "node_repr": self._pin(emb["node_repr"], torch.float32),
-            "edge_repr": self._pin(emb["edge_repr"], torch.float32),
-        }
+        ent = self._entry(_decode(atlas_npz, force_path, vel_path, embed_path), slice(None, kf))
         self._cache[atlas_npz] = ent
         return ent
+
+    def _entry(self, raw: Dict[str, np.ndarray], frames: slice) -> Dict[str, torch.Tensor]:
+        """A decoded protein with the frames ``frames`` of its trajectories, in pinned memory."""
+        return {
+            "atom37": self._pin(raw["all_atom_positions"][frames], torch.float32),           # [T,N,37,3]
+            "force": self._pin(np.asarray(raw["force"])[frames], torch.float64),             # [T,N,3] (the loader's dtype)
+            "vel": self._pin(np.asarray(raw["vel"])[frames], torch.float64),
+            "atom_mask": self._pin(raw["all_atom_mask"], torch.float32),                     # [N,37]
+            "aatype": torch.from_numpy(np.argmax(raw["aatype"], axis=-1)).long(),            # [N]
+            "residue_index": torch.from_numpy(np.asarray(raw["residue_index"])).long(),
+            "node_repr": self._pin(raw["node_repr"], torch.float32),
+            "edge_repr": self._pin(raw["edge_repr"], torch.float32),
+        }
 
     def window_index(self, n_frames: int, training: bool) -> slice:
         """The reference's window arithmetic (:164-190, :214-218), drawing from numpy's global stream exactly as it does.
@@ -120,6 +118,48 @@ class TrajectoryStore:
                 raise ValueError(f"the evaluation window ({t} frames every {k} from frame {start}) reaches past the "
                                  f"{n_frames} frames of the trajectory")
         return slice(start, start + t * k, k)
+
+
+def _decode(atlas_npz: str, force_path: str, vel_path: str, embed_path: str) -> Dict[str, np.ndarray]:
+    """The arrays of one protein's files, named as the loader names them (Dfold_data_loader_dynamic.py:194-198)."""
+    with np.load(atlas_npz, allow_pickle=True) as zf:
+        raw = {k: zf[k] for k in ("all_atom_positions", "all_atom_mask", "aatype", "residue_index")}
+    with open(force_path.replace(".pkl", "_Ca.pkl"), "rb") as f:
+        raw["force"] = pickle.load(f)
+    with open(vel_path.replace(".pkl", "_ca.pkl"), "rb") as f:
+        raw["vel"] = pickle.load(f)
+    with np.load(embed_path) as ef:
+        raw.update({k: ef[k] for k in ("node_repr", "edge_repr")})
+    return raw
+
+
+class EvaluationStore(TrajectoryStore):
+    """The store an evaluation over a test split reads: each protein is decoded when its window is made, only the
+    ``frame_time`` frames of that window (every ``frame_sample_step``-th from ``fix_sample_start``) are pinned, and
+    nothing is kept once the window is built.  A split of many proteins then holds in pinned memory only the windows a
+    ``WindowPrefetcher`` has in flight (at most depth + 1), whatever the length of the trajectories; a ``TrajectoryStore``
+    would keep every trajectory from frame 0 to the end of its window for the life of the store.
+
+    ``protein`` returns an entry whose frame 0 is the window's first frame, and ``window_index`` the whole of it.  A
+    trajectory too short for the window raises the reference loader's ValueError, prefixed with the row's archive."""
+
+    def __init__(self, frame_time: int, frame_sample_step: int = 1, fix_sample_start: int = 0, pin: bool = True):
+        super().__init__(frame_time, frame_sample_step, keep_first=None, fix_sample_start=fix_sample_start, pin=pin)
+
+    def protein(self, atlas_npz: str, force_path: str, vel_path: str, embed_path: str) -> Dict[str, torch.Tensor]:
+        raw = _decode(atlas_npz, force_path, vel_path, embed_path)
+        try:
+            frames = TrajectoryStore.window_index(self, raw["all_atom_positions"].shape[0], training=False)
+        except ValueError as e:
+            raise ValueError(f"{atlas_npz}: {e}") from e
+        return self._entry(raw, frames)
+
+    def window_index(self, n_frames: int, training: bool) -> slice:
+        if training:
+            raise ValueError("an EvaluationStore holds evaluation windows only")
+        if n_frames != self.frame_time:
+            raise ValueError(f"an EvaluationStore entry holds {self.frame_time} frames, not {n_frames}")
+        return slice(0, self.frame_time, 1)
 
 
 class WindowPrefetcher:

@@ -57,19 +57,26 @@ def _int(conf, path: str, low: int, default=KeyError) -> int:
     return int(v)
 
 
+def kept_rows(csv_path: str, max_len, columns: Sequence[str] = ("seq_len",) + ROW_FIELDS) -> List[Dict[str, str]]:
+    """The rows of a split's csv that ``PdbDataset._init_metadata`` keeps (``seq_len <= filtering.max_len``), in csv
+    order, as dicts.  Raises ValueError when one of ``columns`` is absent or when no row is left."""
+    with open(csv_path, newline="") as f:
+        reader = csv.DictReader(f)
+        missing = [k for k in columns if k not in (reader.fieldnames or ())]
+        if missing:
+            raise ValueError(f"{csv_path}: no column {missing}")
+        kept = [r for r in reader if float(r["seq_len"]) <= max_len]
+    if not kept:
+        raise ValueError(f"{csv_path}: no row with seq_len <= {max_len}")
+    return kept
+
+
 def read_rows(csv_path: str, max_len) -> Tuple[List[Tuple[str, str, str, str]], int]:
     """The rows of the training csv that ``PdbDataset._init_metadata`` keeps (``seq_len <= filtering.max_len``), as
     ``TrajectoryStore.protein`` arguments, and their residue count.  Raises ValueError when none is left or when they
     have more than one residue count: one captured step trains one shape."""
-    with open(csv_path, newline="") as f:
-        reader = csv.DictReader(f)
-        missing = [k for k in ("seq_len",) + ROW_FIELDS if k not in (reader.fieldnames or ())]
-        if missing:
-            raise ValueError(f"{csv_path}: no column {missing}")
-        kept = [r for r in reader if float(r["seq_len"]) <= max_len]
+    kept = kept_rows(csv_path, max_len)
     lengths = sorted({float(r["seq_len"]) for r in kept})
-    if not kept:
-        raise ValueError(f"{csv_path}: no row with seq_len <= {max_len}")
     if len(lengths) > 1:
         raise ValueError(f"{csv_path}: the rows with seq_len <= {max_len} have {len(lengths)} residue counts "
                          f"({', '.join(f'{n:g}' for n in lengths)}); the trainer trains proteins of one length")
