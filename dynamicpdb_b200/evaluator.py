@@ -14,10 +14,19 @@ The sampler runs eagerly rather than from one CUDA graph per residue count (``sa
 one window per length, so each captured graph would be replayed once, after a warm-up and a capture that cost more than
 the eager run, and its private memory pool would stay allocated for the rest of the process.
 
+``Evaluator.extend`` is the evaluator's other driver, ``Experiment.eval_extension`` (train_DFOLD_dynamics.py:931-1000),
+made to work over a split: each protein's evaluation window is rolled forward frame by frame
+(``rollout.TrajectoryRollout``, eagerly for the reasons above) and every rollout frame is scored with eval_fn's metrics
+against the MD frame it predicts, which the same ``EvaluationStore`` decode supplies (``horizons``): error against
+horizon.  Rollout frame j predicts MD frame ``fix_sample_start + (frame_time - 1 + j) * frame_sample_step``, because the
+network replaces the window's last frame by the one before it (ipa_pytorch_dynamic.py:819) and the rollout appends each
+prediction as the new last frame (:996).
+
 Not reproduced: the directories, ``eval_conf.yaml``, plots and PDB files eval_fn writes, and the reference's random
 streams (see ``Evaluator``).
 """
 import numbers
+import os
 from typing import Dict, List, Tuple
 
 import numpy as np
@@ -26,13 +35,15 @@ import torch
 from . import checkpoint as _ckpt
 from .inference import DeviceReverseDiffusion
 from .input_pipeline import EvaluationStore, WindowPrefetcher
-from .metrics import eval_sampler_inputs, window_metrics
+from .metrics import HORIZON_KEYS, eval_sampler_inputs, horizon_metrics, window_metrics
+from .rollout import TrajectoryRollout
 from .trainer import ROW_FIELDS, _get, _int, kept_rows
 
 ROW_KEYS = ("ave_rot", "ave_trans", "all_atom_mae", "all_atom_mse", "all_atom_rmsd")   # one device row per window
 PRINTED = (("ave_rot", "ave_rot"), ("ave_trans", "ave_trans"), ("ave_atom_mae", "all_atom_mae"),
            ("ave_atom_rmsd", "all_atom_rmsd"))                                        # eval_fn's summary lines (:925-928)
 MASK_BOUND = 10000.0                                                                  # eval_fn's ``ave_trans < 10000``
+PRINTED_HORIZONS = (1, 10, 100)                        # with the rollout's length: the horizons ``extend`` prints
 
 
 def split_rows(csv_path: str, max_len) -> List[Tuple[str, Tuple[str, str, str, str]]]:
@@ -57,6 +68,15 @@ def load_weights(net: torch.nn.Module, path: str) -> None:
     ckpt = torch.load(path, map_location="cpu", weights_only=False)
     model = _ckpt.check_model(ckpt, {k: v.shape for k, v in net.state_dict().items()})
     net.load_state_dict(model, strict=True)
+
+
+def write_extension(path: str, rigid_traj, atom_traj, aatype) -> None:
+    """eval_extension's ``extension.npz`` (:997-1000) from host arrays: ``atom_traj`` [L, N, 37, 3] and ``rigid_traj``
+    [L, N, 7] float32, and ``aatype``, the window's [nf, N], as the loader's batch of one, [1, nf, N] int64.  The file's
+    directory is made if it does not exist."""
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+    np.savez_compressed(path, atom_traj=np.asarray(atom_traj, dtype=np.float32),
+                        rigid_traj=np.asarray(rigid_traj, dtype=np.float32), aatype=np.asarray(aatype, dtype=np.int64)[None])
 
 
 class Evaluator:
@@ -84,6 +104,7 @@ class Evaluator:
         self.net, self.diffuser, self.seed, self.depth = net, diffuser, int(seed), depth
         self.device = next(net.parameters()).device
         self.sampler = DeviceReverseDiffusion(net)
+        self.roller = TrajectoryRollout(net)
 
     def _configure(self, conf):
         """Everything that needs no device: the config checked, the csv read."""
@@ -120,8 +141,8 @@ class Evaluator:
         """Fresh (windows, reverse steps) generators on the network's device, seeded from ``seed``."""
         return tuple(torch.Generator(self.device).manual_seed(s) for s in eval_seeds(self.seed))
 
-    def _prefetcher(self, generator: torch.Generator):
-        store = EvaluationStore(self.frame_time, self.frame_step, fix_sample_start=self.fix_start)
+    def _prefetcher(self, generator: torch.Generator, horizons: int = 0):
+        store = EvaluationStore(self.frame_time, self.frame_step, fix_sample_start=self.fix_start, horizons=horizons)
         return WindowPrefetcher(store, [row for _, row in self.rows], self.device, training=False, depth=self.depth,
                                 diffuser=self.diffuser, min_t=self.min_t, generator=generator, targets=True)
 
@@ -163,4 +184,63 @@ class Evaluator:
         mask = d["ave_trans"] < MASK_BOUND
         for label, k in PRINTED:
             print(f"{label}:", d[k].sum() / mask.sum())
+        return d
+
+    def extend(self, length: int = 200, out_dir=None) -> Dict[str, object]:
+        """``eval_extension`` over the test split, scored against the MD frames that follow each window.
+
+        For each protein, in csv order: the evaluation window of ``evaluate`` (the same frames, from the same seeded window
+        generator), rolled forward ``length`` frames by ``TrajectoryRollout.rollout(..., graph=False)`` at ``min_t``
+        (200 is eval_extension's hard-coded length, :933); then rollout frame j (horizon j + 1) is scored against MD
+        frame ``fix_sample_start + (frame_time - 1 + j) * frame_sample_step`` with ``metrics.horizon_metrics``: eval_fn's
+        ``ave_rot``, ``ave_trans``, ``all_atom_mae``, ``all_atom_mse`` and ``all_atom_rmsd`` (its ``atom_mask[-1, -1, -1]
+        = 0`` applied to every frame), and ``persist_rot`` / ``persist_trans``, the error of repeating the last MD frame
+        the network was given (window frame ``frame_time - 2``).  Horizon 1 scores the same prediction as ``evaluate``'s
+        row.  A trajectory too short for ``length`` horizons stops the loop; the store's ValueError, naming its archive,
+        is the cause of the prefetcher's error.
+
+        The scores stay in one [n, length, 7] fp64 device tensor read back once, after the last protein.  With ``out_dir``
+        each protein's rollout is also written to ``<out_dir>/<name>/extension.npz`` (``write_extension``, eval_extension's
+        keys, shapes and dtypes), which reads that trajectory back to the host: the only per-protein read.
+
+        Returns {"name": [n names], key: [n, length] fp64 for each of ``HORIZON_KEYS``} and prints, per key, the mean over
+        proteins at horizons 1, 10, 100 and ``length`` (those <= ``length``).  ``length`` and ``out_dir`` are checked
+        before any device work, as the config (``frame_time`` >= 2, which the rollout and ``persist_*`` need) was."""
+        if isinstance(length, bool) or not isinstance(length, int) or length < 1:
+            raise ValueError(f"extend: length must be an int >= 1, got {length!r}")
+        if out_dir is not None and not isinstance(out_dir, (str, bytes)) and not hasattr(out_dir, "__fspath__"):
+            raise ValueError(f"extend: out_dir must be a path or None, got {out_dir!r}")
+        if not self.min_t > 0.0:
+            raise ValueError(f"extend: the rollout runs at data.min_t, which must be > 0, got {self.min_t!r}")
+        return self.summarise_extension(self._read(self._run_extension(length, out_dir)))
+
+    # the device side of the extension loop, replaced by the fixture's scores in the CPU test
+    def _run_extension(self, length: int, out_dir) -> torch.Tensor:
+        """Every protein's ``horizon_metrics`` as one [n, length, 7] fp64 device tensor."""
+        window_gen, _ = self.generators()
+        nf = self.frame_time
+        scores = torch.empty(len(self.rows), length, len(HORIZON_KEYS), dtype=torch.float64, device=self.device)
+        for i, window in enumerate(self._prefetcher(window_gen, horizons=length)):
+            traj = self.roller.rollout(window, length, min_t=float(self.min_t), graph=False)
+            scores[i].copy_(horizon_metrics(traj["rigid_traj"], traj["atom_traj"], window["rigids_0"][nf - 2],
+                                            window["horizon_rigids_0"], window["horizon_atom37_pos"],
+                                            window["horizon_atom37_mask"]))
+            if out_dir is not None:
+                write_extension(os.path.join(os.fsdecode(out_dir), self.names[i], "extension.npz"),
+                                *self._read_trajectory(traj, window))
+        return scores
+
+    def _read_trajectory(self, traj: Dict[str, torch.Tensor], window: Dict[str, torch.Tensor]):
+        """The per-protein device-to-host read of ``extend(out_dir=...)``: (rigid_traj, atom_traj, aatype) as numpy."""
+        return traj["rigid_traj"].cpu().numpy(), traj["atom_traj"].cpu().numpy(), window["aatype"].cpu().numpy()
+
+    def summarise_extension(self, scores: np.ndarray) -> Dict[str, object]:
+        """``extend``'s dict and printed lines from the host scores [n, length, 7] (``HORIZON_KEYS``).  Each printed value
+        is the mean over proteins at one horizon."""
+        d = {"name": list(self.names), **{k: scores[:, :, j].copy() for j, k in enumerate(HORIZON_KEYS)}}
+        length = scores.shape[1]
+        horizons = sorted({h for h in PRINTED_HORIZONS + (length,) if h <= length})
+        for k in HORIZON_KEYS:
+            means = d[k][:, [h - 1 for h in horizons]].mean(axis=0)
+            print(f"{k}:", " ".join(f"h{h} {m}" for h, m in zip(horizons, means)))
         return d

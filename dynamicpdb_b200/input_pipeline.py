@@ -141,15 +141,31 @@ class EvaluationStore(TrajectoryStore):
     would keep every trajectory from frame 0 to the end of its window for the life of the store.
 
     ``protein`` returns an entry whose frame 0 is the window's first frame, and ``window_index`` the whole of it.  A
-    trajectory too short for the window raises the reference loader's ValueError, prefixed with the row's archive."""
+    trajectory too short for the window raises the reference loader's ValueError, prefixed with the row's archive.
 
-    def __init__(self, frame_time: int, frame_sample_step: int = 1, fix_sample_start: int = 0, pin: bool = True):
+    ``horizons=L`` (>= 1) also keeps the MD frames a rollout of ``L`` frames from the window predicts: the entry holds
+    ``frame_time + L - 1`` frames on the same grid (frame ``frame_time - 1 + j`` is the target of rollout frame ``j``),
+    ``window_index`` still names the window's ``frame_time``, and a ``WindowPrefetcher`` adds the targets to each item.  A
+    trajectory too short for ``L`` horizons raises ValueError, prefixed with the row's archive.  0 (the default) keeps the
+    window alone."""
+
+    def __init__(self, frame_time: int, frame_sample_step: int = 1, fix_sample_start: int = 0, pin: bool = True,
+                 horizons: int = 0):
         super().__init__(frame_time, frame_sample_step, keep_first=None, fix_sample_start=fix_sample_start, pin=pin)
+        if isinstance(horizons, bool) or not isinstance(horizons, int) or horizons < 0:
+            raise ValueError(f"horizons must be an int >= 0, got {horizons!r}")
+        self.horizons = horizons
+        self.n_frames = frame_time + max(horizons - 1, 0)
 
     def protein(self, atlas_npz: str, force_path: str, vel_path: str, embed_path: str) -> Dict[str, torch.Tensor]:
         raw = _decode(atlas_npz, force_path, vel_path, embed_path)
+        T = raw["all_atom_positions"].shape[0]
         try:
-            frames = TrajectoryStore.window_index(self, raw["all_atom_positions"].shape[0], training=False)
+            frames = TrajectoryStore.window_index(self, T, training=False)
+            frames = slice(frames.start, frames.start + self.n_frames * self.step, self.step)
+            if frames.start + (self.n_frames - 1) * self.step >= T:
+                raise ValueError(f"{self.horizons} horizons after the evaluation window ({self.n_frames} frames every "
+                                 f"{self.step} from frame {frames.start}) reach past the {T} frames of the trajectory")
         except ValueError as e:
             raise ValueError(f"{atlas_npz}: {e}") from e
         return self._entry(raw, frames)
@@ -157,8 +173,8 @@ class EvaluationStore(TrajectoryStore):
     def window_index(self, n_frames: int, training: bool) -> slice:
         if training:
             raise ValueError("an EvaluationStore holds evaluation windows only")
-        if n_frames != self.frame_time:
-            raise ValueError(f"an EvaluationStore entry holds {self.frame_time} frames, not {n_frames}")
+        if n_frames != self.n_frames:
+            raise ValueError(f"an EvaluationStore entry holds {self.n_frames} frames, not {n_frames}")
         return slice(0, self.frame_time, 1)
 
 
@@ -178,11 +194,18 @@ class WindowPrefetcher:
         and the diffusion draws, default: the device's default generator.  ``targets`` adds the evaluation targets
         ``atom37_pos`` [nf, N, 37, 3] and ``atom37_mask`` [nf, N, 37], fp64 as ``_process_csv_row`` returns them (:249-250),
         which ``metrics.evaluate_window`` scores the sample against (atoms outside the mask keep the archive's coordinates,
-        which the loader zeroes; every metric masks them)."""
+        which the loader zeroes; every metric masks them).
+
+        An ``EvaluationStore(horizons=L)`` with L >= 1 makes each item also carry the targets of a rollout of ``L`` frames
+        from the window, the entry's frames ``frame_time - 1 ..``: ``horizon_rigids_0`` [L, N, 7] fp32,
+        ``horizon_atom37_pos`` [L, N, 37, 3] and ``horizon_atom37_mask`` [L, N, 37], fp64.  The window and its targets come
+        from one copy and one ``featurize_window`` launch over all ``frame_time + L - 1`` frames; the window's fields are
+        its first ``frame_time`` frames and equal, bit for bit, the item made without horizons."""
         dev = torch.device(device)
         if dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device())
         self.store, self.rows, self.device, self.training, self.depth = store, list(rows), dev, training, depth
+        self.horizons = getattr(store, "horizons", 0)
         self.diffuser, self.min_t, self.generator, self.targets = diffuser, float(min_t), generator, bool(targets)
         if not 0.0 <= self.min_t <= 1.0:
             raise ValueError(f"min_t={min_t} outside [0, 1]")
@@ -201,9 +224,20 @@ class WindowPrefetcher:
             # the contiguous frame range straight from the store, whose pinned memory nothing writes; every step-th frame
             # is then taken on the device
             frames = lambda t: cp(t[sl.start:sl.stop])[::sl.step].contiguous()
-            atom37 = frames(ent["atom37"])
             atom_mask = cp(ent["atom_mask"])
-            feats = featurize_window(atom37, atom_mask, cp(ent["aatype"]))
+            if self.horizons:
+                # the window and the frames that follow it, featurised together; the window is their first nf
+                whole = cp(ent["atom37"])
+                feats = featurize_window(whole, atom_mask, cp(ent["aatype"]))
+                horizon = {"horizon_rigids_0": feats["rigids_0"][nf - 1:],
+                           "horizon_atom37_pos": whole[nf - 1:].to(torch.float64),
+                           "horizon_atom37_mask": atom_mask.to(torch.float64).unsqueeze(0).expand(self.horizons, -1, -1)}
+                feats = {k: v[:nf] for k, v in feats.items()}
+                feats.update(horizon)
+                atom37 = whole[:nf]
+            else:
+                atom37 = frames(ent["atom37"])
+                feats = featurize_window(atom37, atom_mask, cp(ent["aatype"]))
             if self.targets:
                 feats["atom37_pos"] = atom37.to(torch.float64)
                 feats["atom37_mask"] = atom_mask.to(torch.float64).unsqueeze(0).expand(nf, -1, -1)

@@ -212,6 +212,41 @@ def window_metrics(rigid_pred: torch.Tensor, atom37_pred: torch.Tensor, rigids_0
             "all_atom_rmsd": rmsd.reshape(1), "per_frame": per_frame}
 
 
+HORIZON_KEYS = ("ave_rot", "ave_trans", "all_atom_mae", "all_atom_mse", "all_atom_rmsd", "persist_rot", "persist_trans")
+
+
+def horizon_metrics(rigid_traj: torch.Tensor, atom_traj: torch.Tensor, last_seen: torch.Tensor, rigids_0: torch.Tensor,
+                    atom37_pos: torch.Tensor, atom37_mask: torch.Tensor, drop_last_atom: bool = True) -> torch.Tensor:
+    """eval_fn's row (``window_metrics``) at every frame of a rollout: [L, 7] fp64 in ``HORIZON_KEYS`` order, row j scoring
+    ``rigid_traj[j]`` [N, 7] / ``atom_traj[j]`` [N, 37, 3] against the MD frame it predicts (``rigids_0[j]``,
+    ``atom37_pos[j]`` under ``atom37_mask[j]``, each [L, ...]).  ``drop_last_atom`` applies eval_fn's ``atom_mask[-1, -1, -1]
+    = 0`` to every frame, as eval_fn applies it to the one frame it scores.  ``persist_rot`` / ``persist_trans`` are the
+    errors of repeating ``last_seen`` [N, 7], the last MD frame the network was given, at every horizon: the
+    ``ref_frame`` baseline of ``rot_trans_error`` with that frame prepended.  Every row is computed by the kernels as
+    ``window_metrics`` computes its last frame, so row 0 of a rollout equals its row bit for bit.  Nothing is read back."""
+    L, N = rigid_traj.shape[:2]
+    A = atom37_pos.shape[2]
+    if rigids_0.shape != rigid_traj.shape or tuple(last_seen.shape) != (N, 7) or atom_traj.shape != atom37_pos.shape \
+            or tuple(atom37_mask.shape) != (L, N, A) or tuple(atom_traj.shape[:2]) != (L, N):
+        raise ValueError(f"horizon_metrics: need rigids [L, N, 7], last_seen [N, 7], atoms [L, N, A, 3] and mask [L, N, A], got "
+                         f"{tuple(rigid_traj.shape)}, {tuple(rigids_0.shape)}, {tuple(last_seen.shape)}, "
+                         f"{tuple(atom_traj.shape)}, {tuple(atom37_pos.shape)}, {tuple(atom37_mask.shape)}")
+    K._need_cuda(rigid_traj, atom_traj, last_seen, rigids_0, atom37_pos, atom37_mask)
+    dev = rigids_0.device
+    with torch.cuda.device(dev):
+        seen = last_seen.unsqueeze(0)
+        gt = torch.cat([seen.to(rigids_0.dtype), rigids_0])
+        pred = torch.cat([seen.to(rigid_traj.dtype), rigid_traj])
+        rot, tr, prot, ptr = rot_trans_error(pred, gt, ref_frame=0)
+        mask = torch.empty(L, N, A, dtype=torch.float64, device=dev).copy_(atom37_mask)
+        if drop_last_atom:
+            mask[:, -1, -1].fill_(0.0)
+        err = atom_errors(atom_traj, atom37_pos, mask)
+        # as window_metrics: the ground truth is moved onto the prediction
+        _, rmsd = superimpose(atom_traj.reshape(L, N * A, 3), atom37_pos.reshape(L, N * A, 3), mask.reshape(L, N * A))
+        return torch.stack([rot[1:], tr[1:], err["mae"], err["mse"], rmsd, prot[1:], ptr[1:]], dim=1)
+
+
 # the sampler inputs eval_fn builds (:826-844) besides the ones it makes itself
 _EVAL_WINDOW_KEYS = ("torsion_angles_sin_cos", "torsion_angles_mask", "node_repr", "edge_repr", "aatype", "rigids_t", "rigids_0",
                      "force", "vel")
