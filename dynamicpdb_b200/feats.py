@@ -86,13 +86,37 @@ def atom14_to_atom37(atom14_data: torch.Tensor, aatype: torch.Tensor):
 _TABLE_NAMES = ("default_frames", "atom14_group", "atom14_mask", "atom14_pos", "atom37_to_atom14", "atom37_mask")
 
 
+def _take(src: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
+    """src [*, G, ...], idx [*, A] -> [*, A, ...]: torch.gather along the G axis as a sum of one-hot selections.  Exact for
+    finite src, and its backward sums in a fixed order, where gather's backward (a scatter_add with atomics) does not."""
+    nb = idx.dim() - 1
+    rest = (1,) * (src.dim() - idx.dim())
+    out = None
+    for g in range(src.shape[nb]):
+        term = (idx == g).to(src.dtype).reshape(idx.shape + rest) * src.select(nb, g).unsqueeze(nb)
+        out = term if out is None else out + term
+    return out
+
+
+def _frames_to_atom14_pos_ordered(r: Rigid, aatype: torch.Tensor) -> torch.Tensor:
+    """frames_to_atom14_pos with _take for its gathers."""
+    dev = r.device
+    grp = table("atom14_group", dev)[aatype, ...]
+    rot14 = _take(r.get_rots().get_rot_mats(), grp)
+    trn14 = _take(r.get_trans(), grp)
+    pos = table("atom14_pos", dev, trn14.dtype)[aatype, ...]
+    out = Rigid(Rotation(rot_mats=rot14), trn14).apply(pos)
+    return out * table("atom14_mask", dev, trn14.dtype)[aatype, ...].unsqueeze(-1)
+
+
 def _eager_chain(rot_is_matrix: bool):
-    """The differentiable statement of the fused kernel (used by its backward): the three reference-shaped functions above."""
+    """The differentiable statement of the fused kernel (used by its backward): the three reference-shaped functions above,
+    with their gathers as fixed-order sums (_take), so that the gradient of atom14 / atom37 is the same from run to run."""
     def run(rot, trans, alpha, aatype, want_frames):
         rots = Rotation(rot_mats=rot) if rot_is_matrix else Rotation(quats=rot, normalize_quats=False)
         frames = torsion_angles_to_frames(Rigid(rots, trans), alpha, aatype, table("default_frames", alpha.device, alpha.dtype))
-        a14 = frames_to_atom14_pos(frames, aatype)
-        a37, _ = atom14_to_atom37(a14, aatype)
+        a14 = _frames_to_atom14_pos_ordered(frames, aatype)
+        a37 = _take(a14, table("atom37_to_atom14", aatype.device)[aatype]) * table("atom37_mask", aatype.device, a14.dtype)[aatype][..., None]
         return (a14, a37, frames.to_tensor_4x4()) if want_frames else (a14, a37)
     return run
 

@@ -67,6 +67,7 @@ _SIGS = {
     "dfold_lr_schedule": "p" + "dd" + "lll" + "d" + "pp",
     "dfold_featurize_window": "pppppp" + "ii" + "pppp" + "p",
     "dfold_loss_fwd": "pppppppppppp" + "ii" + "dddd" + "ii" + "pppp" + "p",
+    "dfold_aux_loss_fwd": "ppppp" + "iii" + "ddddd" + "pppp" + "p",
     "dfold_quat_mul_fwd": "ppplip",
     "dfold_quat_mul_bwd": "ppppplip",
     "dfold_rot_compose_fwd": "pppp" + "pp" + "liip",
@@ -107,7 +108,7 @@ def exported_symbols():
 
 # kernels launched per C-ABI call (bench.py reports the total as `gpu_launches`)
 _LAUNCHES_PER_CALL = {"dfold_global_layernorm_fwd": 3, "dfold_global_layernorm_bwd": 3, "dfold_ipa_attn_bwd": 4,
-                      "dfold_grad_norm": 2}
+                      "dfold_grad_norm": 2, "dfold_aux_loss_fwd": 2}
 LAUNCH_COUNT = 0
 # When True (set by train_step.TrainStep around its step), weight gradients of the convolution are accumulated by the kernel
 # straight into the parameter's existing .grad buffer and autograd receives None: the ConvNet is shared by the four blocks

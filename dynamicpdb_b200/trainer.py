@@ -26,11 +26,13 @@ from torch.utils.data.distributed import DistributedSampler
 
 from . import checkpoint as _ckpt
 from .input_pipeline import TrajectoryStore, WindowPrefetcher
-from .loss import score_network_loss
+from .loss import AUX_KEYS, aux_conf, score_network_loss
 from .train_step import TrainStep
 
 ROW_FIELDS = ("atlas_npz", "force_path", "vel_path", "embed_path")
 LOGGED = ("total_loss", "rot_loss", "trans_loss", "torsion_loss")     # score_network_loss's aux_data keys without 'batch'
+# with aux_losses=True, in the reference's aux_data order (train_DFOLD_dynamics.py:1384-1390)
+LOGGED_AUX = ("total_loss", "rot_loss", "trans_loss", "bb_atom_loss", "dist_mat_loss", "torsion_loss")
 
 _log = logging.getLogger(__name__)
 
@@ -115,16 +117,22 @@ class Trainer:
     it, which is not reproduced, and neither is the per-rank stream of the ranks ``accumulate`` stands in for.
 
     ``graph=False`` runs eager steps (a gloo process group cannot be captured); ``max_grad_norm`` and ``lr_schedule`` are
-    ``TrainStep``'s."""
+    ``TrainStep``'s.
+
+    ``aux_losses=True`` trains on the objective with the backbone-atom and pair-distance losses added
+    (``score_network_loss(aux_losses=True)``); ``experiment.bb_atom_loss_weight``, ``bb_atom_loss_t_filter``,
+    ``dist_mat_loss_weight``, ``dist_mat_loss_t_filter`` and ``aux_loss_weight`` must then be numbers, and the log line
+    carries ``bb_atom_loss`` and ``dist_mat_loss`` too, in the reference's order."""
 
     def __init__(self, conf, net: torch.nn.Module, diffuser, *, world_size: int = 1, rank: int = 0, accumulate: int = 1,
-                 graph: bool = True, warmup: int = 3, max_grad_norm: Optional[float] = None, lr_schedule=None):
-        self._configure(conf, world_size, rank, accumulate)
+                 graph: bool = True, warmup: int = 3, max_grad_norm: Optional[float] = None, lr_schedule=None,
+                 aux_losses: bool = False):
+        self._configure(conf, world_size, rank, accumulate, aux_losses=aux_losses)
         self._build(net, diffuser, graph=graph, warmup=warmup, max_grad_norm=max_grad_norm, lr_schedule=lr_schedule)
         np.random.seed(rank)
         torch.manual_seed(rank)
 
-    def _configure(self, conf, world_size: int, rank: int, accumulate: int):
+    def _configure(self, conf, world_size: int, rank: int, accumulate: int, aux_losses: bool = False):
         """Everything that needs no device: the config checked, the csv read."""
         self.conf = conf
         for name, v, low in (("world_size", world_size, 1), ("accumulate", accumulate, 1), ("rank", rank, 0)):
@@ -150,6 +158,12 @@ class Trainer:
             raise ValueError(f"experiment.learning_rate must be a non-negative number, got {self.lr!r}")
         self.exp_conf = types.SimpleNamespace(**{k: _get(conf, "experiment." + k) for k in (
             "torsion_loss_weight", "rot_loss_weight", "trans_loss_weight", "rot_loss_t_threshold", "separate_rot_loss")})
+        self.aux_losses = bool(aux_losses)
+        self.logged_keys = LOGGED_AUX if self.aux_losses else LOGGED
+        if self.aux_losses:
+            for k in AUX_KEYS:
+                setattr(self.exp_conf, k, _get(conf, "experiment." + k))
+            aux_conf(self.exp_conf)
         self.diffuse_rot = bool(_get(conf, "diffuser.diffuse_rot", True))
         self.frame_time = _int(conf, "data.frame_time", 1)
         self.frame_step = _int(conf, "data.frame_sample_step", 1)
@@ -173,10 +187,10 @@ class Trainer:
         example, = list(WindowPrefetcher(self.store, self.rows[:1], self.device, diffuser=diffuser, min_t=self.min_t))
         self.step = TrainStep(net, self._loss, example, lr=float(self.lr), world_size=self.world, accumulate=self.accumulate,
                               loss_reads_window=True, **step_kw)
-        self.logged = torch.zeros(len(LOGGED), dtype=torch.float64, device=self.device)
+        self.logged = torch.zeros(len(self.logged_keys), dtype=torch.float64, device=self.device)
 
     def _loss(self, out, window):
-        return score_network_loss(out, window, self.exp_conf, self.diffuse_rot)
+        return score_network_loss(out, window, self.exp_conf, self.diffuse_rot, aux_losses=self.aux_losses)
 
     def windows(self, epoch: int) -> List[List[int]]:
         """The dataset indices of this rank's slots at every step of `epoch`: ``[step][slot]``."""
@@ -192,7 +206,7 @@ class Trainer:
 
     def _keep_logged(self):
         """The values this step logs: one device-to-device copy of TrainStep.aux, read at the next log line."""
-        self.logged.copy_(torch.stack([self.step.aux[k].to(torch.float64) for k in LOGGED]))
+        self.logged.copy_(torch.stack([self.step.aux[k].to(torch.float64) for k in self.logged_keys]))
 
     def _read_logged(self) -> List[float]:
         return self.logged.tolist()
@@ -234,7 +248,7 @@ class Trainer:
                 values = self._read_logged()
                 elapsed = time.time() - log_time
                 log_time = time.time()
-                losses = " ".join(f"{k}={v:.4f}" for k, v in zip(LOGGED, values))
+                losses = " ".join(f"{k}={v:.4f}" for k, v in zip(self.logged_keys, values))
                 _log.info(f"Epoch[{self.trained_epochs}/{self.num_epoch}] trained_steps: [{self.trained_steps}]: "
                           f"{losses}, steps/sec={self.log_freq / elapsed:.5f}")
                 keep = True

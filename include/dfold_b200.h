@@ -318,6 +318,15 @@ int dfold_loss_fwd(const double* ang, const double* a_gt, const double* a_alt, c
                    const double* gt_rot, const double* x, const double* x0, const double* res_mask, const double* fixed_mask,
                    const double* t, const double* rot_scaling, int nf, int N, double w_tor, double w_rot, double w_trans,
                    double t_thr, int rot_on, int separate, double* out, double* d_ang, double* d_rs, double* d_x, void* stream);
+/* Auxiliary structure losses (csrc/aux_loss.cu), the backbone-atom MSE and the < 6 A pair-distance loss of
+ * Experiment.loss_fn (train_DFOLD_dynamics.py:1316-1364, normalised as :1374-1375), over EVERY frame, in two launches and
+ * no O((5N)^2) buffer.  pred_atom37 / gt_atom37 [nf,N,37,3] fp32 (atoms 0..4 = N, CA, C, CB, O read); masks [nf,N] fp64;
+ * t[f * t_stride] (t_stride 0 or 1) gates frame f by t < t_bb / t < t_dm on the device.  work: nf * ceil(5N / 128) * 5
+ * fp64.  out[2 + 2 nf] = {bb_atom_loss, dist_mat_loss (normalised), bb_atom_loss[nf], dist_mat_loss[nf]};
+ * d_bb / d_dm [nf,N,5,3] fp64 = d out[0] / d pred and d out[1] / d pred (atoms 0..4).  nf <= 2048. */
+int dfold_aux_loss_fwd(const float* pred_atom37, const float* gt_atom37, const double* res_mask, const double* fixed_mask,
+                       const double* t, int t_stride, int nf, int N, double w_bb, double t_bb, double w_dm, double t_dm,
+                       double w_aux, double* work, double* out, double* d_bb, double* d_dm, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Input featurisation of a trajectory window (csrc/featurize.cu), SURVEY.md 8 f4: atom37 coordinates [nf,N,37,3] ->
