@@ -67,6 +67,35 @@ class DFOLDv2_Embeder(nn.Module):
         return node_embed, edge_embed.reshape(num_batch, num_res, num_res, -1), node_embed[0], ref_edge, t_embed
 
 
+def check_windows(feats_list) -> None:
+    """The windows ``FullScoreNetwork.forward_windows`` takes: a non-empty list of input dicts with the same keys and,
+    key by key, the same shape and dtype; in particular the same residue and frame counts.  Raises ValueError."""
+    if not isinstance(feats_list, (list, tuple)) or not feats_list:
+        raise ValueError("forward_windows: needs a non-empty list of window dicts")
+    if not all(isinstance(f, dict) for f in feats_list):
+        raise ValueError("forward_windows: every window must be a dict of input tensors")
+    f0 = feats_list[0]
+    for k in ("node_repr", "rigids_0"):
+        if k not in f0:
+            raise ValueError(f"forward_windows: window 0 has no '{k}'")
+    n0, nf0 = f0["node_repr"].shape[0], f0["rigids_0"].shape[0]
+    for i, f in enumerate(feats_list[1:], start=1):
+        if set(f) != set(f0):
+            raise ValueError(f"forward_windows: window {i} has keys {sorted(set(f) ^ set(f0))} that window 0 "
+                             "has not, or the reverse")
+        n, nf = f["node_repr"].shape[0], f["rigids_0"].shape[0]
+        if n != n0:
+            raise ValueError(f"forward_windows: window {i} has {n} residues and window 0 has {n0}; one pass takes "
+                             "windows of one residue count")
+        if nf != nf0:
+            raise ValueError(f"forward_windows: window {i} has {nf} frames and window 0 has {nf0}; one pass takes "
+                             "windows of one frame count")
+        for k, v in f.items():
+            if torch.is_tensor(v) and (v.shape != f0[k].shape or v.dtype != f0[k].dtype):
+                raise ValueError(f"forward_windows: '{k}' of window {i} is {tuple(v.shape)} {v.dtype}, of window 0 "
+                                 f"{tuple(f0[k].shape)} {f0[k].dtype}")
+
+
 class FullScoreNetwork(nn.Module):
     """ref :429-569."""
 
@@ -120,6 +149,49 @@ class FullScoreNetwork(nn.Module):
         pred_out["atom14"] = atom14_pos
         pred_out["rigid_update"] = model_out["rigid_update"]
         return pred_out
+
+    def forward_windows(self, feats_list):
+        """``[forward(f) for f in feats_list]`` in one pass: the windows' per-frame inputs are stacked along the frame axis,
+        so every row-wise layer (``expand_*``, the embedders' linears, AngleResnet, BackboneUpdate, ``frames_to_atoms``)
+        and every convolution runs once for all of them, while each window is normalised, convolved and scored on its own
+        (``DFOLDIpaScore.forward_windows``).  IPA runs once per window.  The windows may come from different proteins, but
+        must share their residue count, frame count and the shape and dtype of every input; anything else raises
+        ValueError before any device work.  Returns one output dict per window, with ``forward``'s keys; its tensors are
+        views of the stacked results.  Like ``forward``, it stores ``expand_node_repr`` / ``expand_edge_repr`` in each
+        window's dict."""
+        check_windows(feats_list)
+        W = len(feats_list)
+        f0 = feats_list[0]
+        num_res = f0["node_repr"].shape[0]
+        nf = f0["rigids_0"].shape[0]
+        node = K.linear(torch.cat([f["node_repr"] for f in feats_list], dim=0), self.expand_node.weight,
+                        self.expand_node.bias)
+        edge = K.linear(torch.cat([f["edge_repr"].reshape(num_res * num_res, -1) for f in feats_list], dim=0),
+                        self.expand_edge.weight, self.expand_edge.bias)
+        for i, f in enumerate(feats_list):
+            f["expand_node_repr"] = node[i * num_res:(i + 1) * num_res]
+            f["expand_edge_repr"] = edge[i * num_res * num_res:(i + 1) * num_res * num_res].reshape(num_res, num_res, -1)
+
+        model_out = self.score_model.forward_windows(feats_list)
+
+        gt_angles = torch.cat([f["torsion_angles_sin_cos"] for f in feats_list], dim=0)
+        dm = 1 - torch.cat([f["fixed_mask"] for f in feats_list], dim=0).type(torch.float32)[..., None, None]
+        angles_pred = self._apply_mask(model_out["angles"], gt_angles, dm)
+        unorm_angles = self._apply_mask(model_out["unorm_angles"], gt_angles, dm)
+        rigids_pred = model_out["final_rigids"]
+        atom14_pos, atom37_pos = feats.frames_to_atoms(rigids_pred, angles_pred,
+                                                       torch.cat([f["aatype"] for f in feats_list], dim=0))
+        stacked = {
+            "angles": angles_pred,
+            "unorm_angles": unorm_angles,
+            "rot_score": model_out["rot_score"],
+            "trans_score": model_out["trans_score"],
+            "rigids": rigids_pred.to_tensor_7(),
+            "atom37": atom37_pos,
+            "atom14": atom14_pos,
+            "rigid_update": model_out["rigid_update"],
+        }
+        return [{k: v[i * nf:(i + 1) * nf] for k, v in stacked.items()} for i in range(W)]
 
     def debug_foward(self, input_feats, drop_ref=False):
         """ref :549-569: forward + the set of parameters whose module ran."""

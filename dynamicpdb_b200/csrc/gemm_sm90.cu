@@ -71,6 +71,12 @@ struct GemmParams {
     int a_f_mul, a_z_mul;   // A outer coordinate = f * a_f_mul + zq * a_z_mul
     int b_f_mul, b_z_mul;   // B outer coordinate = f * b_f_mul + zq * b_z_mul (+ df)
     int b_n_zmul;           // B column offset    = zq * b_n_zmul
+    // ---- stacked windows (0: 3-D operand maps, the plain path) ----
+    // windows > 0: the activation maps gain a 4th (window) dimension; the frame halo is zero-filled at every window's edge.
+    // mode 0: row tiles run window-major, win_tiles per window, output rows (w * F_out + f) * Nr + n.
+    // mode 1: the k-blocks run window-major, win_kb per window.
+    int windows;
+    int win_tiles, win_fout, win_kb;
     long long* stats;       // debug (dfold_debug_gemm_stats): per CTA {total, consumer wait full, producer wait empty, 0} cycles
 };
 
@@ -103,6 +109,17 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
         ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(bar) : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
+        ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar) : "memory");
+}
+// A / B tile load of the producer: 3-D maps, or with stacked windows 4-D maps whose outer coordinate is the window
+__device__ __forceinline__ void tma_load(bool win, uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2,
+                                         int w) {
+    if (win) tma_load_4d(dst, map, bar, c0, c1, c2, w);
+    else tma_load_3d(dst, map, bar, c0, c1, c2);
 }
 
 // 128B-swizzled operand tile descriptors (sm_90 wgmma layout: start >> 4 in [0,14), LBO in [16,30), SBO in [32,46),
@@ -296,11 +313,14 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
     const int n_tile = blockIdx.x;                 // output column tile
     const int m_tile = blockIdx.y;
     const int zq = (p.mode == 1) ? (int)blockIdx.z : 0;       // mode 1: tap or batch id
-    int f0 = 0, n0 = 0, m0 = 0, hb = 0;
+    int f0 = 0, n0 = 0, m0 = 0, hb = 0, win = 0;
     const int num_kb = p.num_kb;
+    const bool wmap = p.windows > 0;
     if (p.mode == 0) {
-        f0 = m_tile / p.tiles_per_frame;
-        n0 = (m_tile % p.tiles_per_frame) * BM;
+        const int mt = wmap ? m_tile % p.win_tiles : m_tile;
+        win = wmap ? m_tile / p.win_tiles : 0;
+        f0 = mt / p.tiles_per_frame;
+        n0 = (mt % p.tiles_per_frame) * BM;
         hb = f0 % p.bmod;
     } else {
         m0 = m_tile * BM;
@@ -336,15 +356,17 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
                     const int af = f0 / p.a_f_div + p.f_start + df;
                     const int bk = c * BK + p.b_k_ofs + hb * p.b_k_bstride;
                     const int bz = tap + hb * p.b_z_bstride;
-                    tma_load_3d(sa_hi, &map_a_hi, full_bar(s), ak, n0 + dn, af);
-                    tma_load_3d(sa_lo, &map_a_lo, full_bar(s), ak, n0 + dn, af);
+                    tma_load(wmap, sa_hi, &map_a_hi, full_bar(s), ak, n0 + dn, af, win);
+                    tma_load(wmap, sa_lo, &map_a_lo, full_bar(s), ak, n0 + dn, af, win);
                     tma_load_3d(sb_hi, &map_b_hi, full_bar(s), bk, col0, bz);
                     tma_load_3d(sb_lo, &map_b_lo, full_bar(s), bk, col0, bz);
                 } else {
                     // K runs over pixels (f, 64-residue block j); operands are MN-major: boxes of
                     // 64 channels x 64 residues, one per 64-wide channel atom.  The tap shift is on the
                     // residue / frame coordinates (row dimensions), out-of-image rows are zero-filled.
-                    const int f = kb / p.kc, j = kb % p.kc;
+                    const int kw = wmap ? kb % p.win_kb : kb;
+                    const int wk = wmap ? kb / p.win_kb : 0;
+                    const int f = kw / p.kc, j = kw % p.kc;
                     const bool has_taps = p.taps_n * p.taps_f > 1;
                     const int dn = has_taps ? zq % p.taps_n - p.taps_n / 2 : 0;
                     const int df = has_taps ? zq / p.taps_n - p.taps_f / 2 : 0;
@@ -353,13 +375,13 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
                     const int bn0 = col0 + zq * p.b_n_zmul;
 #pragma unroll
                     for (int a = 0; a < BM / 64; ++a) {
-                        tma_load_3d(sa_hi + a * 8192, &map_a_hi, full_bar(s), m0 + a * 64, j * BK, af);
-                        tma_load_3d(sa_lo + a * 8192, &map_a_lo, full_bar(s), m0 + a * 64, j * BK, af);
+                        tma_load(wmap, sa_hi + a * 8192, &map_a_hi, full_bar(s), m0 + a * 64, j * BK, af, wk);
+                        tma_load(wmap, sa_lo + a * 8192, &map_a_lo, full_bar(s), m0 + a * 64, j * BK, af, wk);
                     }
 #pragma unroll
                     for (int b = 0; b < BN / 64; ++b) {
-                        tma_load_3d(sb_hi + b * 8192, &map_b_hi, full_bar(s), bn0 + b * 64, j * BK + dn, bf);
-                        tma_load_3d(sb_lo + b * 8192, &map_b_lo, full_bar(s), bn0 + b * 64, j * BK + dn, bf);
+                        tma_load(wmap, sb_hi + b * 8192, &map_b_hi, full_bar(s), bn0 + b * 64, j * BK + dn, bf, wk);
+                        tma_load(wmap, sb_lo + b * 8192, &map_b_lo, full_bar(s), bn0 + b * 64, j * BK + dn, bf, wk);
                     }
                 }
             }
@@ -401,7 +423,7 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_co
             bool row_ok;
             if (p.mode == 0) {
                 const int n = n0 + r;
-                grow = (long)(f0 / p.o_f_div) * p.Nr + n;
+                grow = ((long)win * p.win_fout + f0 / p.o_f_div) * p.Nr + n;
                 row_ok = (n < p.Nr) && (grow < p.out_rows);
             } else {
                 grow = m0 + r;
@@ -457,21 +479,26 @@ EncodeTiledFn get_encode() {
     return fn;
 }
 
-// bf16 tensor with dims d0 (innermost, contiguous), d1, d2; strides in ELEMENTS for d1, d2.
-int make_map(CUtensorMap* m, const void* base, long d0, long d1, long d2, long s1, long s2, int b0, int b1, int b2) {
+// bf16 tensor with dims d0 (innermost, contiguous), d1, d2 and, when d3 > 0, d3; strides in ELEMENTS for d1, d2, d3.
+// The box spans one element of d2 and d3.
+int make_map(CUtensorMap* m, const void* base, long d0, long d1, long d2, long s1, long s2, int b0, int b1, int b2,
+             long d3 = 0, long s3 = 0) {
     EncodeTiledFn enc = get_encode();
     DFOLD_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled unavailable (driver too old?)");
     DFOLD_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "TMA base pointer must be 16-byte aligned");
-    DFOLD_REQUIRE((s1 * 2) % 16 == 0 && (s2 * 2) % 16 == 0, "TMA strides must be multiples of 16 bytes (s1=%ld s2=%ld)", s1, s2);
-    cuuint64_t dims[3] = {(cuuint64_t)d0, (cuuint64_t)d1, (cuuint64_t)d2};
-    cuuint64_t strides[2] = {(cuuint64_t)s1 * 2, (cuuint64_t)s2 * 2};
-    cuuint32_t box[3] = {(cuuint32_t)b0, (cuuint32_t)b1, (cuuint32_t)b2};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
+    DFOLD_REQUIRE((s1 * 2) % 16 == 0 && (s2 * 2) % 16 == 0 && (s3 * 2) % 16 == 0,
+                  "TMA strides must be multiples of 16 bytes (s1=%ld s2=%ld s3=%ld)", s1, s2, s3);
+    const cuuint32_t rank = d3 > 0 ? 4 : 3;
+    cuuint64_t dims[4] = {(cuuint64_t)d0, (cuuint64_t)d1, (cuuint64_t)d2, (cuuint64_t)d3};
+    cuuint64_t strides[3] = {(cuuint64_t)s1 * 2, (cuuint64_t)s2 * 2, (cuuint64_t)s3 * 2};
+    cuuint32_t box[4] = {(cuuint32_t)b0, (cuuint32_t)b1, (cuuint32_t)b2, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(base), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    DFOLD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) dims=(%ld,%ld,%ld) strides=(%ld,%ld) box=(%d,%d,%d)",
-                  (int)r, d0, d1, d2, s1, s2, b0, b1, b2);
+    DFOLD_REQUIRE(r == CUDA_SUCCESS,
+                  "cuTensorMapEncodeTiled failed (%d) dims=(%ld,%ld,%ld,%ld) strides=(%ld,%ld,%ld) box=(%d,%d,%d)",
+                  (int)r, d0, d1, d2, d3, s1, s2, s3, b0, b1, b2);
     return 0;
 }
 
@@ -503,6 +530,7 @@ void default_batching(GemmParams& p) {
     p.bmod = 1; p.a_f_div = 1; p.a_k_bstride = 0; p.b_k_ofs = 0; p.b_k_bstride = 0; p.b_z_bstride = 0;
     p.o_f_div = 1; p.o_col_bstride = 0; p.f_start = 0; p.b_f_add = 0;
     p.a_f_mul = 1; p.a_z_mul = 0; p.b_f_mul = 1; p.b_z_mul = 0; p.b_n_zmul = 0;
+    p.windows = 0; p.win_tiles = 0; p.win_fout = 0; p.win_kb = 0;
 }
 
 
@@ -538,19 +566,22 @@ extern "C" int dfold_debug_gemm_stats(long long* buf) {
 namespace dfold {
 namespace {
 
-// dfold_gemm_bf16x3 on tiles `bn` wide.  `name`: the calling entry point, for error messages.
-int gemm_kmajor(const char* name, const uint16_t* a_hi, const uint16_t* a_lo, long F, long F_out, int f_start, long Nr,
-                long K, long lda, const uint16_t* b_hi, const uint16_t* b_lo, long n_out, long ldb, int taps_f, int taps_n,
-                float* out, long ldo, const float* bias, const float* residual, long ldr,
+// dfold_gemm_bf16x3 on tiles `bn` wide.  `name`: the calling entry point, for error messages.  W > 0: W stacked windows
+// of F frames each (dfold_gemm_bf16x3_windows); W = 0: one image of F frames on 3-D maps.
+int gemm_kmajor(const char* name, const uint16_t* a_hi, const uint16_t* a_lo, long W, long F, long F_out, int f_start,
+                long Nr, long K, long lda, const uint16_t* b_hi, const uint16_t* b_lo, long n_out, long ldb, int taps_f,
+                int taps_n, float* out, long ldo, const float* bias, const float* residual, long ldr,
                 float alpha, float beta, int act, int bn, void* stream) {
-    DFOLD_REQUIRE(F > 0 && F_out > 0 && Nr > 0 && K > 0 && n_out > 0, "%s: empty problem", name);
+    DFOLD_REQUIRE(F > 0 && F_out > 0 && Nr > 0 && K > 0 && n_out > 0 && W >= 0, "%s: empty problem", name);
     DFOLD_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "%s: lda/ldb must be multiples of 8 (got %ld, %ld)", name, lda, ldb);
     DFOLD_REQUIRE(taps_f >= 1 && taps_n >= 1 && (taps_f & 1) && (taps_n & 1), "%s: tap grid must be odd", name);
     DFOLD_REQUIRE(bn == 64 || bn == 128, "%s: tile width must be 64 or 128 (got %d)", name, bn);
+    const long row_tiles = F_out * cdiv(Nr, BM);
+    DFOLD_REQUIRE((W > 0 ? W : 1) * row_tiles <= 65535, "%s: too many row tiles (%ld)", name, (W > 0 ? W : 1) * row_tiles);
     CUtensorMap maps[4];
-    // A: dims (K, Nr, F)   B: dims (K, n_out, taps)
-    if (make_map(&maps[0], a_hi, K, Nr, F, lda, Nr * lda, BK, BM, 1)) return 1;
-    if (make_map(&maps[1], a_lo, K, Nr, F, lda, Nr * lda, BK, BM, 1)) return 1;
+    // A: dims (K, Nr, F [, W])   B: dims (K, n_out, taps)
+    if (make_map(&maps[0], a_hi, K, Nr, F, lda, Nr * lda, BK, BM, 1, W, F * Nr * lda)) return 1;
+    if (make_map(&maps[1], a_lo, K, Nr, F, lda, Nr * lda, BK, BM, 1, W, F * Nr * lda)) return 1;
     const long taps = (long)taps_f * taps_n;
     if (make_map(&maps[2], b_hi, K, n_out, taps, ldb, n_out * ldb, BK, bn, 1)) return 1;
     if (make_map(&maps[3], b_lo, K, n_out, taps, ldb, n_out * ldb, BK, bn, 1)) return 1;
@@ -561,39 +592,41 @@ int gemm_kmajor(const char* name, const uint16_t* a_hi, const uint16_t* a_lo, lo
     p.taps_n = taps_n; p.taps_f = taps_f;
     p.tiles_per_frame = (int)cdiv(Nr, BM);
     p.Nr = (int)Nr;
-    p.out_rows = F_out * Nr;
+    p.out_rows = (W > 0 ? W : 1) * F_out * Nr;
     p.n_out = (int)n_out;
     p.out = out; p.ldo = ldo; p.out_tap_stride = 0;
     p.bias = bias; p.res = residual; p.ldr = ldr;
     p.alpha = alpha; p.beta = beta; p.act = act;
     default_batching(p);
     p.f_start = f_start;
+    p.windows = (int)W; p.win_tiles = (int)row_tiles; p.win_fout = (int)F_out;
     cudaStream_t st = as_stream(stream);
     // Every output element is produced by one CTA in a fixed k order (no split-K with atomics): the result is the same
-    // from run to run, and the same at either tile width.
-    dim3 grid((unsigned)cdiv(n_out, bn), (unsigned)(F_out * p.tiles_per_frame), 1);
+    // from run to run, and the same at either tile width.  A row tile lies in one frame of one window.
+    dim3 grid((unsigned)cdiv(n_out, bn), (unsigned)((W > 0 ? W : 1) * row_tiles), 1);
     if (bn == 128) return launch<128>(maps, p, grid, st);
     return launch<64>(maps, p, grid, st);
 }
 
-// dfold_gemm_wgrad_bf16x3 on tiles `bn` wide.
+// dfold_gemm_wgrad_bf16x3 on tiles `bn` wide.  W > 0: the reduction runs over the pixels of W stacked windows, window
+// by window (dfold_gemm_wgrad_bf16x3_windows); W = 0: one image on 3-D maps.
 int gemm_wgrad(const char* name, const uint16_t* a_hi, const uint16_t* a_lo, long M, long lda,
                const uint16_t* b_hi, const uint16_t* b_lo, long Nn, long ldb,
-               long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
+               long W, long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
                float* out, long ldo, float alpha, int bn, void* stream) {
-    DFOLD_REQUIRE(M > 0 && Nn > 0 && F > 0 && Fb > 0 && Nr > 0, "%s: empty problem", name);
+    DFOLD_REQUIRE(M > 0 && Nn > 0 && F > 0 && Fb > 0 && Nr > 0 && W >= 0, "%s: empty problem", name);
     DFOLD_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "%s: lda/ldb must be multiples of 8 (got %ld, %ld)", name, lda, ldb);
     DFOLD_REQUIRE(bn == 64 || bn == 128, "%s: tile width must be 64 or 128 (got %d)", name, bn);
     CUtensorMap maps[4];
-    // dims (channel, residue, frame); boxes of 64 channels x 64 residues
-    if (make_map(&maps[0], a_hi, M, Nr, F, lda, Nr * lda, 64, BK, 1)) return 1;
-    if (make_map(&maps[1], a_lo, M, Nr, F, lda, Nr * lda, 64, BK, 1)) return 1;
-    if (make_map(&maps[2], b_hi, Nn, Nr, Fb, ldb, Nr * ldb, 64, BK, 1)) return 1;
-    if (make_map(&maps[3], b_lo, Nn, Nr, Fb, ldb, Nr * ldb, 64, BK, 1)) return 1;
+    // dims (channel, residue, frame [, window]); boxes of 64 channels x 64 residues
+    if (make_map(&maps[0], a_hi, M, Nr, F, lda, Nr * lda, 64, BK, 1, W, F * Nr * lda)) return 1;
+    if (make_map(&maps[1], a_lo, M, Nr, F, lda, Nr * lda, 64, BK, 1, W, F * Nr * lda)) return 1;
+    if (make_map(&maps[2], b_hi, Nn, Nr, Fb, ldb, Nr * ldb, 64, BK, 1, W, Fb * Nr * ldb)) return 1;
+    if (make_map(&maps[3], b_lo, Nn, Nr, Fb, ldb, Nr * ldb, 64, BK, 1, W, Fb * Nr * ldb)) return 1;
     GemmParams p{};
     p.mode = 1;
     p.kc = (int)cdiv(Nr, BK);
-    p.num_kb = (int)(F * p.kc);
+    p.num_kb = (int)((W > 0 ? W : 1) * F * p.kc);
     p.taps_n = taps_n; p.taps_f = taps_f;
     p.tiles_per_frame = 1; p.Nr = (int)Nr;
     p.out_rows = M; p.n_out = (int)Nn;
@@ -602,6 +635,7 @@ int gemm_wgrad(const char* name, const uint16_t* a_hi, const uint16_t* a_lo, lon
     p.alpha = alpha; p.beta = 0.f; p.act = 0;
     default_batching(p);
     p.b_f_add = b_f_add;
+    p.windows = (int)W; p.win_kb = (int)(F * p.kc);
     dim3 grid((unsigned)cdiv(Nn, bn), (unsigned)cdiv(M, BM), (unsigned)(taps_f * taps_n));
     cudaStream_t st = as_stream(stream);
     if (bn == 128) return launch<128>(maps, p, grid, st);
@@ -616,7 +650,7 @@ extern "C" int dfold_gemm_bf16x3(
     const uint16_t* b_hi, const uint16_t* b_lo, long n_out, long ldb, int taps_f, int taps_n,
     float* out, long ldo, const float* bias, const float* residual, long ldr,
     float alpha, float beta, int act, void* stream) {
-    return gemm_kmajor("dfold_gemm_bf16x3", a_hi, a_lo, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f,
+    return gemm_kmajor("dfold_gemm_bf16x3", a_hi, a_lo, 0, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f,
                        taps_n, out, ldo, bias, residual, ldr, alpha, beta, act, pick_bn(n_out, F_out * cdiv(Nr, BM)), stream);
 }
 
@@ -626,7 +660,7 @@ extern "C" int dfold_gemm_bf16x3_bn(
     const uint16_t* b_hi, const uint16_t* b_lo, long n_out, long ldb, int taps_f, int taps_n,
     float* out, long ldo, const float* bias, const float* residual, long ldr,
     float alpha, float beta, int act, int bn, void* stream) {
-    return gemm_kmajor("dfold_gemm_bf16x3_bn", a_hi, a_lo, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f,
+    return gemm_kmajor("dfold_gemm_bf16x3_bn", a_hi, a_lo, 0, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f,
                        taps_n, out, ldo, bias, residual, ldr, alpha, beta, act, bn, stream);
 }
 
@@ -639,7 +673,7 @@ extern "C" int dfold_gemm_wgrad_bf16x3(
     const uint16_t* b_hi, const uint16_t* b_lo, long Nn, long ldb,
     long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
     float* out, long ldo, float alpha, void* stream) {
-    return gemm_wgrad("dfold_gemm_wgrad_bf16x3", a_hi, a_lo, M, lda, b_hi, b_lo, Nn, ldb, F, Fb, b_f_add, Nr, taps_f, taps_n,
+    return gemm_wgrad("dfold_gemm_wgrad_bf16x3", a_hi, a_lo, M, lda, b_hi, b_lo, Nn, ldb, 0, F, Fb, b_f_add, Nr, taps_f, taps_n,
                       out, ldo, alpha, pick_bn(Nn, cdiv(M, BM) * taps_f * taps_n), stream);
 }
 
@@ -649,8 +683,32 @@ extern "C" int dfold_gemm_wgrad_bf16x3_bn(
     const uint16_t* b_hi, const uint16_t* b_lo, long Nn, long ldb,
     long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
     float* out, long ldo, float alpha, int bn, void* stream) {
-    return gemm_wgrad("dfold_gemm_wgrad_bf16x3_bn", a_hi, a_lo, M, lda, b_hi, b_lo, Nn, ldb, F, Fb, b_f_add, Nr, taps_f,
+    return gemm_wgrad("dfold_gemm_wgrad_bf16x3_bn", a_hi, a_lo, M, lda, b_hi, b_lo, Nn, ldb, 0, F, Fb, b_f_add, Nr, taps_f,
                       taps_n, out, ldo, alpha, bn, stream);
+}
+
+// dfold_gemm_bf16x3_bn over W >= 1 stacked windows: A planes [W][F][Nr][lda], output / residual rows (w * F_out + f) * Nr + n.
+// Each window is convolved on its own: the frame halo is zero-filled at every window's edge.
+extern "C" int dfold_gemm_bf16x3_windows(
+    const uint16_t* a_hi, const uint16_t* a_lo, long W, long F, long F_out, int f_start, long Nr, long K, long lda,
+    const uint16_t* b_hi, const uint16_t* b_lo, long n_out, long ldb, int taps_f, int taps_n,
+    float* out, long ldo, const float* bias, const float* residual, long ldr,
+    float alpha, float beta, int act, int bn, void* stream) {
+    DFOLD_REQUIRE(W >= 1, "dfold_gemm_bf16x3_windows: need at least one window (got %ld)", W);
+    return gemm_kmajor("dfold_gemm_bf16x3_windows", a_hi, a_lo, W, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb,
+                       taps_f, taps_n, out, ldo, bias, residual, ldr, alpha, beta, act, bn, stream);
+}
+
+// dfold_gemm_wgrad_bf16x3_bn summed over W >= 1 stacked windows: A planes [W][F][Nr][lda], B planes [W][Fb][Nr][ldb];
+// frame f of A's window w pairs with frame f + b_f_add of B's window w, and taps never reach into another window.
+extern "C" int dfold_gemm_wgrad_bf16x3_windows(
+    const uint16_t* a_hi, const uint16_t* a_lo, long M, long lda,
+    const uint16_t* b_hi, const uint16_t* b_lo, long Nn, long ldb,
+    long W, long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
+    float* out, long ldo, float alpha, int bn, void* stream) {
+    DFOLD_REQUIRE(W >= 1, "dfold_gemm_wgrad_bf16x3_windows: need at least one window (got %ld)", W);
+    return gemm_wgrad("dfold_gemm_wgrad_bf16x3_windows", a_hi, a_lo, M, lda, b_hi, b_lo, Nn, ldb, W, F, Fb, b_f_add, Nr,
+                      taps_f, taps_n, out, ldo, alpha, bn, stream);
 }
 
 // Batched K-major GEMM (no taps): for every row tile of "frame" b in [0, n_batches), hb = b % bmod:

@@ -290,8 +290,15 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const SgemmParams p) {
 // ---------------------------------------------------------------------------------------------------
 // whole-tensor layer norm (MyLayerNorm, reference ipa_pytorch_dynamic.py:709-724)
 // ---------------------------------------------------------------------------------------------------
+// Segments: S tensors of n elements each, normalised one by one in one launch per pass.  Segment s is blockIdx.y of
+// the element-wise passes (blockIdx.x of the one-block reductions); each segment sees exactly the grid, partition and
+// order of a single-tensor launch of n elements.  Workspace: segment s's block partials at [s * 2048, s * 2048 + 2048),
+// its backward sums at S * 2048 + 2 s.
+constexpr long kGlnPartials = 2048;
 // pass 1: per-block partial (sum, sum of squares about a shift) in double -> partial[2*blocks]
 __global__ void gln_partial_kernel(const float* __restrict__ x, long n, double* __restrict__ partial) {
+    x += (long)blockIdx.y * n;
+    partial += (long)blockIdx.y * kGlnPartials;
     double s = 0.0, q = 0.0;
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
         const double v = (double)x[i];
@@ -311,6 +318,8 @@ __global__ void gln_partial_kernel(const float* __restrict__ x, long n, double* 
 }
 // pass 2 (one block): stats[0] = mean, stats[1] = 1/sqrt(var_unbiased + eps)
 __global__ void gln_finalize_kernel(const double* __restrict__ partial, int nblocks, long n, float eps, float* __restrict__ stats) {
+    partial += (long)blockIdx.x * kGlnPartials;
+    stats += 2 * blockIdx.x;
     double s = 0.0, q = 0.0;
     for (int i = threadIdx.x; i < nblocks; i += blockDim.x) { s += partial[2 * i]; q += partial[2 * i + 1]; }
     __shared__ double ss[32], qq[32];
@@ -329,6 +338,9 @@ __global__ void gln_finalize_kernel(const double* __restrict__ partial, int nblo
 }
 __device__ __forceinline__ float silu_f(float v) { return v / (1.f + expf(-v)); }
 __global__ void gln_apply_kernel(const float* __restrict__ x, const float* __restrict__ stats, float* __restrict__ y, long n, int silu) {
+    x += (long)blockIdx.y * n;
+    y += (long)blockIdx.y * n;
+    stats += 2 * blockIdx.y;
     const float mean = stats[0], rstd = stats[1];
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
         float v = (x[i] - mean) * rstd;
@@ -340,6 +352,10 @@ __global__ void gln_apply_kernel(const float* __restrict__ x, const float* __res
 //   dx = rstd * (g - mean(g) - xhat * sum(g*xhat)/(n-1))
 __global__ void gln_bwd_partial_kernel(const float* __restrict__ x, const float* __restrict__ dy, const float* __restrict__ stats,
                                        long n, int silu, double* __restrict__ partial) {
+    x += (long)blockIdx.y * n;
+    dy += (long)blockIdx.y * n;
+    stats += 2 * blockIdx.y;
+    partial += (long)blockIdx.y * kGlnPartials;
     const float mean = stats[0], rstd = stats[1];
     double s = 0.0, q = 0.0;
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
@@ -361,6 +377,8 @@ __global__ void gln_bwd_partial_kernel(const float* __restrict__ x, const float*
     }
 }
 __global__ void gln_bwd_reduce_kernel(const double* __restrict__ partial, int nblocks, double* __restrict__ sums) {
+    partial += (long)blockIdx.x * kGlnPartials;
+    sums += 2 * blockIdx.x;
     double s = 0.0, q = 0.0;
     for (int i = threadIdx.x; i < nblocks; i += blockDim.x) { s += partial[2 * i]; q += partial[2 * i + 1]; }
     __shared__ double ss[32], qq[32];
@@ -376,6 +394,11 @@ __global__ void gln_bwd_reduce_kernel(const double* __restrict__ partial, int nb
 }
 __global__ void gln_bwd_apply_kernel(const float* __restrict__ x, const float* __restrict__ dy, const float* __restrict__ stats,
                                      const double* __restrict__ sums, float* __restrict__ dx, long n, int silu) {
+    x += (long)blockIdx.y * n;
+    dy += (long)blockIdx.y * n;
+    dx += (long)blockIdx.y * n;
+    stats += 2 * blockIdx.y;
+    sums += 2 * blockIdx.y;
     const float mean = stats[0], rstd = stats[1];
     const float gmean = (float)(sums[0] / (double)n);
     const float gx = (float)(sums[1] / (double)(n > 1 ? n - 1 : 1));
@@ -586,25 +609,52 @@ extern "C" int dfold_sgemm(const float* A, long a_rs, long a_cs, long a_bs, long
     return check_launch("sgemm_kernel");
 }
 
-// workspace: at least 2*1024 + 2 doubles
-extern "C" int dfold_global_layernorm_fwd(const float* x, float* y, float* stats, double* workspace, long n, float eps, int silu, void* stream) {
-    DFOLD_REQUIRE(n > 1, "dfold_global_layernorm_fwd: need at least 2 elements");
+namespace {
+// the block partition of every segment is chosen from n alone, as for one tensor of n elements
+int gln_fwd(const char* name, const float* x, float* y, float* stats, double* workspace, long n, int segments, float eps,
+            int silu, cudaStream_t st) {
+    DFOLD_REQUIRE(n > 1, "%s: need at least 2 elements per segment", name);
+    DFOLD_REQUIRE(segments >= 1 && segments <= 65535, "%s: segments must be in [1, 65535] (got %d)", name, segments);
     const int blocks = (int)(cdiv(n, 256 * 8) < 1024 ? cdiv(n, 256 * 8) : 1024);
-    cudaStream_t st = as_stream(stream);
-    gln_partial_kernel<<<blocks, 256, 0, st>>>(x, n, workspace);
-    gln_finalize_kernel<<<1, 256, 0, st>>>(workspace, blocks, n, eps, stats);
-    gln_apply_kernel<<<(int)(cdiv(n, 256 * 4) < 4096 ? cdiv(n, 256 * 4) : 4096), 256, 0, st>>>(x, stats, y, n, silu);
+    const int ablocks = (int)(cdiv(n, 256 * 4) < 4096 ? cdiv(n, 256 * 4) : 4096);
+    gln_partial_kernel<<<dim3(blocks, segments), 256, 0, st>>>(x, n, workspace);
+    gln_finalize_kernel<<<segments, 256, 0, st>>>(workspace, blocks, n, eps, stats);
+    gln_apply_kernel<<<dim3(ablocks, segments), 256, 0, st>>>(x, stats, y, n, silu);
     return check_launch("global_layernorm_fwd");
 }
 
-extern "C" int dfold_global_layernorm_bwd(const float* x, const float* dy, const float* stats, double* workspace, float* dx, long n, int silu, void* stream) {
-    DFOLD_REQUIRE(n > 1, "dfold_global_layernorm_bwd: need at least 2 elements");
+int gln_bwd(const char* name, const float* x, const float* dy, const float* stats, double* workspace, float* dx, long n,
+            int segments, int silu, cudaStream_t st) {
+    DFOLD_REQUIRE(n > 1, "%s: need at least 2 elements per segment", name);
+    DFOLD_REQUIRE(segments >= 1 && segments <= 65535, "%s: segments must be in [1, 65535] (got %d)", name, segments);
     const int blocks = (int)(cdiv(n, 256 * 8) < 1024 ? cdiv(n, 256 * 8) : 1024);
-    cudaStream_t st = as_stream(stream);
-    gln_bwd_partial_kernel<<<blocks, 256, 0, st>>>(x, dy, stats, n, silu, workspace);
-    gln_bwd_reduce_kernel<<<1, 256, 0, st>>>(workspace, blocks, workspace + 2048);
-    gln_bwd_apply_kernel<<<(int)(cdiv(n, 256 * 4) < 4096 ? cdiv(n, 256 * 4) : 4096), 256, 0, st>>>(x, dy, stats, workspace + 2048, dx, n, silu);
+    const int ablocks = (int)(cdiv(n, 256 * 4) < 4096 ? cdiv(n, 256 * 4) : 4096);
+    double* sums = workspace + (long)segments * kGlnPartials;
+    gln_bwd_partial_kernel<<<dim3(blocks, segments), 256, 0, st>>>(x, dy, stats, n, silu, workspace);
+    gln_bwd_reduce_kernel<<<segments, 256, 0, st>>>(workspace, blocks, sums);
+    gln_bwd_apply_kernel<<<dim3(ablocks, segments), 256, 0, st>>>(x, dy, stats, sums, dx, n, silu);
     return check_launch("global_layernorm_bwd");
+}
+}  // namespace
+
+// workspace: at least 2*1024 + 2 doubles
+extern "C" int dfold_global_layernorm_fwd(const float* x, float* y, float* stats, double* workspace, long n, float eps, int silu, void* stream) {
+    return gln_fwd("dfold_global_layernorm_fwd", x, y, stats, workspace, n, 1, eps, silu, as_stream(stream));
+}
+
+extern "C" int dfold_global_layernorm_bwd(const float* x, const float* dy, const float* stats, double* workspace, float* dx, long n, int silu, void* stream) {
+    return gln_bwd("dfold_global_layernorm_bwd", x, dy, stats, workspace, dx, n, 1, silu, as_stream(stream));
+}
+
+// `segments` tensors of n elements each, one after the other: stats [segments][2]; workspace >= segments * 2050 doubles
+extern "C" int dfold_global_layernorm_seg_fwd(const float* x, float* y, float* stats, double* workspace, long n, int segments,
+                                              float eps, int silu, void* stream) {
+    return gln_fwd("dfold_global_layernorm_seg_fwd", x, y, stats, workspace, n, segments, eps, silu, as_stream(stream));
+}
+
+extern "C" int dfold_global_layernorm_seg_bwd(const float* x, const float* dy, const float* stats, double* workspace, float* dx,
+                                              long n, int segments, int silu, void* stream) {
+    return gln_bwd("dfold_global_layernorm_seg_bwd", x, dy, stats, workspace, dx, n, segments, silu, as_stream(stream));
 }
 
 extern "C" int dfold_row_layernorm_fwd(const float* x, const float* w, const float* b, float* y, float* stats, long rows, int C, float eps, void* stream) {

@@ -196,19 +196,25 @@ class ConvNet(nn.Module):
                 nn.Conv2d(dim, dim // 2, kernel_size=5, padding=2), nn.ReLU(True),
                 nn.Conv2d(dim // 2, dim, kernel_size=5, padding=2), nn.ReLU(True)))
 
-    def forward(self, x, last_frame_only: bool = False):
+    def forward(self, x, last_frame_only: bool = False, windows: Optional[int] = None):
         """x [frames, residues, dim] -> same shape.
 
         ``last_frame_only`` (needs >= 17 frames): returns [1, residues, dim], the LAST frame of the full result, computing
-        for each of the eight layers only the frames that last frame still depends on (15, 13, ... 1)."""
+        for each of the eight layers only the frames that last frame still depends on (15, 13, ... 1).
+
+        ``windows=W``: x stacks W windows of equal frame counts, each convolved on its own (``kernels.conv5x5``); with
+        ``last_frame_only`` the result is [W, residues, dim], the last frame of each window."""
+        # the plain calls keep the operators' plain signatures (the CPU tests route them to the oracle's ops)
+        win = {} if windows is None else {"windows": windows}
         for st in range(1, 5):
             seq = getattr(self, f"conv{st}")
             if last_frame_only:
-                h = K.conv5x5(x, seq[0].weight, seq[0].bias, relu=True, crop=2)
-                x = K.conv5x5(h, seq[2].weight, seq[2].bias, relu=True, residual=x[4:], crop=2)
+                h = K.conv5x5(x, seq[0].weight, seq[0].bias, relu=True, crop=2, **win)
+                res = x[4:] if windows is None else x.unflatten(0, (windows, -1))[:, 4:].flatten(0, 1)
+                x = K.conv5x5(h, seq[2].weight, seq[2].bias, relu=True, residual=res, crop=2, **win)
             else:
-                h = K.conv5x5(x, seq[0].weight, seq[0].bias, relu=True)
-                x = K.conv5x5(h, seq[2].weight, seq[2].bias, relu=True, residual=x)
+                h = K.conv5x5(x, seq[0].weight, seq[0].bias, relu=True, **win)
+                x = K.conv5x5(h, seq[2].weight, seq[2].bias, relu=True, residual=x, **win)
         return x
 
 
@@ -220,8 +226,9 @@ class MyLayerNorm(nn.Module):
         super().__init__()
         self.eps = 1e-4
 
-    def forward(self, x):
-        return K.global_layernorm(x, self.eps)
+    def forward(self, x, segments: Optional[int] = None):
+        """``segments=W``: x stacks W windows along its leading axis, each normalised on its own."""
+        return K.global_layernorm(x, self.eps, **({} if segments is None else {"segments": segments}))
 
 
 class TimeBlock(nn.Module):
@@ -266,11 +273,12 @@ def _embedder(in_dim: int, width: int) -> nn.Sequential:
     return nn.Sequential(nn.Linear(in_dim, width), nn.SiLU(), nn.Linear(width, width), MyLayerNorm(), nn.SiLU())
 
 
-def _run_embedder(seq: nn.Sequential, x: torch.Tensor) -> torch.Tensor:
-    """Linear-SiLU-Linear-MyLayerNorm-SiLU (ref :757-796) on the fused kernels."""
+def _run_embedder(seq: nn.Sequential, x: torch.Tensor, windows: Optional[int] = None) -> torch.Tensor:
+    """Linear-SiLU-Linear-MyLayerNorm-SiLU (ref :757-796) on the fused kernels; ``windows=W``: x stacks W windows along
+    its leading axis and the layer norm takes one mean / variance per window."""
     h = K.linear(x, seq[0].weight, seq[0].bias, act="silu")
     h = K.linear(h, seq[2].weight, seq[2].bias)
-    return K.global_layernorm(h, seq[3].eps, silu=True)
+    return K.global_layernorm(h, seq[3].eps, silu=True, **({} if windows is None else {"segments": windows}))
 
 
 def _shift_last(x: torch.Tensor) -> torch.Tensor:
@@ -386,5 +394,84 @@ class DFOLDIpaScore(nn.Module):
             "rot_score": rot_score,
             "trans_score": trans_score,
             "final_rigids": curr_rigids,
+            "rigid_update": rigid_update,
+        }
+
+    def forward_windows(self, feats_list):
+        """``forward`` over W windows of equal frame and residue counts in one pass (checked by the caller,
+        ``FullScoreNetwork.forward_windows``).  The per-frame inputs are stacked along the frame axis, and the row-wise
+        layers run once on all W * nf frames.  What couples frames stays within a window: ``_shift_last``, the
+        last-frame-only ``rigid_update``, each window's own index embedding and node / edge representations, one
+        MyLayerNorm mean and variance per window, the ConvNet's frame halo (and the dead-frame crop), and ``t`` in the
+        score epilogue.  IPA runs once per window.  Returns the stacked trunk outputs, with ``final_rigids`` a Rigid over
+        all W * nf frames; window i owns frames [i * nf, (i + 1) * nf) of every entry."""
+        W = len(feats_list)
+        f0 = feats_list[0]
+        nf = f0["rigids_0"].shape[0]
+        cat = lambda xs: torch.cat(xs, dim=0)
+        node_mask = [f["res_mask"].type(torch.float32) for f in feats_list]
+        diffuse_mask = cat([(1 - f["fixed_mask"].type(torch.float32)) * m for f, m in zip(feats_list, node_mask)])
+        init_rigids = [Rigid.from_tensor_7(f["rigids_t"].type(torch.float32)) for f in feats_list]
+        dt = f0["rigids_0"].dtype
+        curr = cat([_shift_last(f["rigids_0"]).to(torch.float32) for f in feats_list])
+
+        force_embed = _run_embedder(self.force_embeder, cat([_shift_last(f["force"].to(dt)) for f in feats_list]), W)
+        vel_embed = _run_embedder(self.vel_embeder, cat([_shift_last(f["vel"].to(dt)) for f in feats_list]), W)
+
+        idx = cat([f["seq_idx"][0:1].unsqueeze(-1).to(f["node_repr"].dtype) for f in feats_list])      # [W,N,1]
+        node_1 = _run_embedder(self.index_embeder, idx, W)
+        node_embed = [(node_1[i] + f["expand_node_repr"]).unsqueeze(0).expand(nf, -1, -1) for i, f in enumerate(feats_list)]
+
+        angle = []
+        for f in feats_list:
+            a = f["torsion_angles_sin_cos"].to(dt)
+            a = (a * f["torsion_angles_mask"].to(dt).unsqueeze(-1)).to(dt)
+            angle.append(_shift_last(a).reshape(nf, -1, a.shape[-2] * 2))
+        angle_embed = _run_embedder(self.angle_embeder, cat(angle), W)
+
+        node_feat = init_node_feat = rigid_update = None
+        for b in range(self._ipa_conf.num_blocks):
+            rigids_embed = _run_embedder(self.rigid_embeder, curr, W)
+            ipa = self.trunk[f"ipa_{b}"]
+            ipa_embed = cat([ipa(node_embed[i], f["expand_edge_repr"], Rigid.from_tensor_7(curr[i * nf:(i + 1) * nf]),
+                                 node_mask[i]) for i, f in enumerate(feats_list)])
+            ipa_embed = self.trunk[f"ln_{b}"](ipa_embed, segments=W)
+            node_feat = torch.cat([rigids_embed, ipa_embed, force_embed, vel_embed, angle_embed], dim=-1)
+            halo = 2 * 8                        # dead-frame elimination, per window (see forward)
+            middle = (0 < b < self._ipa_conf.num_blocks - 1) and nf > halo + 1 and _DEAD_FRAME_SKIP
+            if middle:
+                tail = node_feat.unflatten(0, (W, nf))[:, -(halo + 1):].flatten(0, 1)
+                node_feat = self.trunk["conv_0"](tail, last_frame_only=True, windows=W)                  # [W,N,5c]
+                last = node_feat
+            else:
+                node_feat = self.trunk["conv_0"](node_feat, windows=W)
+                last = node_feat.unflatten(0, (W, nf))[:, -1]
+            upd_last = self.trunk[f"bb_update_{b}"](last)                                                 # [W,N,6]
+            rigid_update = torch.cat([upd_last.new_zeros((W, nf - 1) + upd_last.shape[1:]), upd_last[:, None]],
+                                     dim=1).flatten(0, 1)
+            new_rigids = Rigid.from_tensor_7(curr).compose_q_update_vec(rigid_update, diffuse_mask[..., None])
+            curr = new_rigids.to_tensor_7()
+            if b == 0:
+                init_node_feat = node_feat
+
+        unorm_angles, angles = self.angle_resnet(node_feat, init_node_feat)
+        rot_score, trans_score = [], []
+        for i, f in enumerate(feats_list):
+            cr = Rigid.from_tensor_7(curr[i * nf:(i + 1) * nf])
+            if self._fused_scores is not None:
+                rs, ts = self._fused_scores.fused_scores(init_rigids[i], cr, f["t"], node_mask[i],
+                                                         self._ipa_conf.coordinate_scaling)
+            else:
+                rs = self.diffuser.calc_rot_score(init_rigids[i].get_rots(), cr.get_rots(), f["t"]) * node_mask[i][..., None]
+                ts = self.diffuser.calc_trans_score(init_rigids[i].get_trans(), self.unscale_rigids(cr).get_trans(),
+                                                    f["t"][:, None, None], use_torch=True) * node_mask[i][..., None]
+            rot_score.append(rs)
+            trans_score.append(ts)
+        return {
+            "angles": angles,
+            "unorm_angles": unorm_angles,
+            "rot_score": cat(rot_score),
+            "trans_score": cat(trans_score),
+            "final_rigids": self.unscale_rigids(Rigid.from_tensor_7(curr)),
             "rigid_update": rigid_update,
         }

@@ -37,6 +37,8 @@ _SIGS = {
     "dfold_sgemm": "pllll" * 4 + "p" + "iiiii" + "ff" + "iii" + "p",
     "dfold_global_layernorm_fwd": "pppplfip",
     "dfold_global_layernorm_bwd": "pppppl" + "ip",
+    "dfold_global_layernorm_seg_fwd": "ppppl" + "ifip",
+    "dfold_global_layernorm_seg_bwd": "pppppl" + "iip",
     "dfold_row_layernorm_fwd": "ppppplifp",
     "dfold_row_layernorm_bwd": "ppppppplip",
     "dfold_quat_to_rot_fwd": "pplp",
@@ -49,6 +51,8 @@ _SIGS = {
     "dfold_gemm_bf16x3_bn": "pplli" + "lll" + "ppllii" + "pl" + "p" + "pl" + "ffi" + "i" + "p",
     "dfold_gemm_wgrad_bf16x3": "ppll" + "ppll" + "llilii" + "plf" + "p",
     "dfold_gemm_wgrad_bf16x3_bn": "ppll" + "ppll" + "llilii" + "plf" + "i" + "p",
+    "dfold_gemm_bf16x3_windows": "ppllli" + "lll" + "ppllii" + "pl" + "p" + "pl" + "ffi" + "i" + "p",
+    "dfold_gemm_wgrad_bf16x3_windows": "ppll" + "ppll" + "lllilii" + "plf" + "i" + "p",
     "dfold_ipa_attn_fwd": "plplppplpppp" + "iiiiiiii" + "ff" + "ppp",
     "dfold_ipa_attn_bwd": "plplppplpppp" + "iiiiiiii" + "ff" + "ppp" + "ppppppppp" + "p",
     "dfold_ipa_pre_bwd": "pp" + "iiiiiii" + "pp" + "pppp" + "p",
@@ -108,6 +112,7 @@ def exported_symbols():
 
 # kernels launched per C-ABI call (bench.py reports the total as `gpu_launches`)
 _LAUNCHES_PER_CALL = {"dfold_global_layernorm_fwd": 3, "dfold_global_layernorm_bwd": 3, "dfold_ipa_attn_bwd": 4,
+                      "dfold_global_layernorm_seg_fwd": 3, "dfold_global_layernorm_seg_bwd": 3,
                       "dfold_grad_norm": 2, "dfold_aux_loss_fwd": 2}
 LAUNCH_COUNT = 0
 # When True (set by train_step.TrainStep around its step), weight gradients of the convolution are accumulated by the kernel
@@ -377,24 +382,34 @@ def _conv_bn(n_out: int, row_tiles: int, dev) -> int:
 
 
 def _gemm(a_hi, a_lo, F, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f, taps_n, out, ldo, bias, residual, ldr, alpha, beta, act,
-          F_out=None, f_start=0, bn=None):
-    """dfold_gemm_bf16x3, or with ``bn`` set its explicit-width form dfold_gemm_bf16x3_bn."""
+          F_out=None, f_start=0, bn=None, windows=None):
+    """dfold_gemm_bf16x3, or with ``bn`` set its explicit-width form dfold_gemm_bf16x3_bn, or with ``windows`` (and ``bn``)
+    set dfold_gemm_bf16x3_windows over that many stacked windows of F frames each."""
     F_out = F if F_out is None else F_out
     args = (a_hi, a_lo, F, F_out, f_start, Nr, K, lda, b_hi, b_lo, n_out, ldb, taps_f, taps_n, out, ldo, bias, residual, ldr,
             alpha, beta, act)
-    with _timed("gemm_bf16x3", 2.0 * F_out * Nr * K * n_out * taps_f * taps_n, f"kmajor F{F_out} N{Nr} K{K} out{n_out} taps{taps_f * taps_n}"):
-        if bn is None:
+    W = windows or 1
+    with _timed("gemm_bf16x3", 2.0 * W * F_out * Nr * K * n_out * taps_f * taps_n,
+                f"kmajor W{W} F{F_out} N{Nr} K{K} out{n_out} taps{taps_f * taps_n}"):
+        if windows is not None:
+            launch("dfold_gemm_bf16x3_windows", a_hi, a_lo, windows, *args[2:], bn)
+        elif bn is None:
             launch("dfold_gemm_bf16x3", *args)
         else:
             launch("dfold_gemm_bf16x3_bn", *args, bn)
 
 
-def _gemm_wgrad(a, M, lda, b, Nn, ldb, F, Nr, taps_f, taps_n, out, ldo, Fb=None, b_f_add=0, bn=None):
-    """dfold_gemm_wgrad_bf16x3, or with ``bn`` set dfold_gemm_wgrad_bf16x3_bn."""
+def _gemm_wgrad(a, M, lda, b, Nn, ldb, F, Nr, taps_f, taps_n, out, ldo, Fb=None, b_f_add=0, bn=None, windows=None):
+    """dfold_gemm_wgrad_bf16x3, or with ``bn`` set dfold_gemm_wgrad_bf16x3_bn, or with ``windows`` (and ``bn``) set
+    dfold_gemm_wgrad_bf16x3_windows, summed over that many stacked windows."""
     Fb = F if Fb is None else Fb
     args = (a[0], a[1], M, lda, b[0], b[1], Nn, ldb, F, Fb, b_f_add, Nr, taps_f, taps_n, out, ldo, 1.0)
-    with _timed("gemm_bf16x3", 2.0 * F * Nr * M * Nn * taps_f * taps_n, f"wgrad F{F} N{Nr} M{M} n{Nn} taps{taps_f * taps_n}"):
-        if bn is None:
+    W = windows or 1
+    with _timed("gemm_bf16x3", 2.0 * W * F * Nr * M * Nn * taps_f * taps_n,
+                f"wgrad W{W} F{F} N{Nr} M{M} n{Nn} taps{taps_f * taps_n}"):
+        if windows is not None:
+            launch("dfold_gemm_wgrad_bf16x3_windows", *args[:8], windows, *args[8:], bn)
+        elif bn is None:
             launch("dfold_gemm_wgrad_bf16x3", *args)
         else:
             launch("dfold_gemm_wgrad_bf16x3_bn", *args, bn)
@@ -506,35 +521,39 @@ def linear(x, weight, bias=None, act: Optional[str] = None, residual=None, pre_r
 class _Conv5x5Fn(Function):
     @staticmethod
     @_on_device
-    def forward(ctx, x, w, b, relu, residual, crop):
+    def forward(ctx, x, w, b, relu, residual, crop, windows):
         _need_cuda(x, w, b, residual)
-        F_, N_, Ci = x.shape
+        FW, N_, Ci = x.shape
         Co, Ci2, kh, kw = w.shape
         if Ci2 != Ci or Ci % 8 or Co % 8:
             raise ValueError(f"conv5x5: channels must match and be multiples of 8 (got {Ci}->{Co})")
-        Fo = F_ - crop                                   # only the last Fo frames are produced
+        W = windows or 1
+        F_ = FW // W                                     # frames per window
+        Fo = F_ - crop                                   # only the last Fo frames of each window are produced
         if Fo < 1:
             raise ValueError("conv5x5: crop removes every frame")
-        x2 = _f32c(x.reshape(F_ * N_, Ci))
-        r2 = _f32c(residual.reshape(Fo * N_, Co)) if residual is not None else None
-        out = torch.empty((Fo * N_, Co), dtype=torch.float32, device=x.device)
+        x2 = _f32c(x.reshape(FW * N_, Ci))
+        r2 = _f32c(residual.reshape(W * Fo * N_, Co)) if residual is not None else None
+        out = torch.empty((W * Fo * N_, Co), dtype=torch.float32, device=x.device)
         (a_hi, a_lo), _ = _split2d(x2)
         f_hi, f_lo, _, _ = _conv_planes(w)
         _gemm(a_hi, a_lo, F_, N_, Ci, Ci, f_hi, f_lo, Co, f_hi.shape[2], kh, kw, out, Co, _f32c(b) if b is not None else None,
-              r2, Co, 1.0, 1.0, 1 if relu else 0, F_out=Fo, f_start=crop, bn=_conv_bn(Co, Fo * -(-N_ // 128), x.device))
+              r2, Co, 1.0, 1.0, 1 if relu else 0, F_out=Fo, f_start=crop,
+              bn=_conv_bn(Co, W * Fo * -(-N_ // 128), x.device), windows=windows)
         ctx.save_for_backward(a_hi, a_lo, w, out if relu else None, r2 if relu else None)
-        ctx.meta = (x.shape, relu, b is not None, residual is not None, crop)
+        ctx.meta = ((F_, N_, Ci), relu, b is not None, residual is not None, crop, windows)
         ctx.w_param = w if isinstance(w, torch.nn.Parameter) else None
-        return out.reshape(Fo, N_, Co)
+        return out.reshape(W * Fo, N_, Co)
 
     @staticmethod
     @_on_device
     def backward(ctx, dy):
         x_hi, x_lo, w, out, r2 = ctx.saved_tensors
-        (F_, N_, Ci), relu, has_b, has_r, crop = ctx.meta
+        (F_, N_, Ci), relu, has_b, has_r, crop, windows = ctx.meta
         Co, _, kh, kw = w.shape
+        W = windows or 1
         Fo = F_ - crop
-        g = _f32c(dy.reshape(Fo * N_, Co))
+        g = _f32c(dy.reshape(W * Fo * N_, Co))
         need_x, need_w, need_b = ctx.needs_input_grad[0], ctx.needs_input_grad[1], has_b and ctx.needs_input_grad[2]
         dx = dw = db = None
         db_buf = torch.zeros(Co, dtype=torch.float32, device=g.device) if need_b else None
@@ -546,7 +565,7 @@ class _Conv5x5Fn(Function):
             if not (acc is not None and acc.dtype == torch.float32 and acc.is_contiguous() and acc.shape == w.shape
                     and acc.device == g.device):
                 acc = None
-        wgrad = lambda out_, add: _conv_wgrad(g_hi, g_lo, x_hi, x_lo, Co, Ci, kh, kw, F_, Fo, N_, crop, out_, add)
+        wgrad = lambda out_, add: _conv_wgrad(g_hi, g_lo, x_hi, x_lo, Co, Ci, kh, kw, F_, Fo, N_, crop, out_, add, windows)
         side = acc is not None and PROFILE is None
         if side:
             # the weight gradient only adds into the parameter's .grad: it overlaps the data gradient and the rest of the
@@ -555,32 +574,50 @@ class _Conv5x5Fn(Function):
                 wgrad(acc, 1)
         if need_x:
             _, _, d_hi, d_lo = _conv_planes(w)
-            dx = torch.empty((F_ * N_, Ci), dtype=torch.float32, device=g.device)
+            dx = torch.empty((W * F_ * N_, Ci), dtype=torch.float32, device=g.device)
             _gemm(g_hi, g_lo, Fo, N_, Co, Co, d_hi, d_lo, Ci, d_hi.shape[2], kh, kw, dx, Ci, None, None, 0, 1.0, 0.0, 0,
-                  F_out=F_, f_start=-crop, bn=_conv_bn(Ci, F_ * -(-N_ // 128), g.device))
-            dx = dx.reshape(F_, N_, Ci)
+                  F_out=F_, f_start=-crop, bn=_conv_bn(Ci, W * F_ * -(-N_ // 128), g.device), windows=windows)
+            dx = dx.reshape(W * F_, N_, Ci)
         if acc is not None and not side:
             wgrad(acc, 1)
         elif need_w and acc is None:
             dw = torch.empty((Co, Ci, kh, kw), dtype=torch.float32, device=g.device)
             wgrad(dw, 0)
-        return dx, dw, db, None, (dy if has_r else None), None
+        return dx, dw, db, None, (dy if has_r else None), None, None
 
 
-def _conv_wgrad(g_hi, g_lo, x_hi, x_lo, Co, Ci, kh, kw, F_, Fo, N_, crop, out, add):
+def _conv_wgrad(g_hi, g_lo, x_hi, x_lo, Co, Ci, kh, kw, F_, Fo, N_, crop, out, add, windows=None):
     """Weight gradient of the convolution: the per-tap GEMMs into a [taps, Co, Ci] scratch (allocated on the current
-    stream), then added into (add=1) or written to (add=0) ``out`` [Co, Ci, kh, kw]."""
+    stream), then added into (add=1) or written to (add=0) ``out`` [Co, Ci, kh, kw].  With ``windows``, one launch sums
+    the gradient over that many stacked windows of F_ input (Fo output) frames each."""
     taps = torch.empty((kh * kw, Co, Ci), dtype=torch.float32, device=out.device)
     _gemm_wgrad((g_hi, g_lo), Co, Co, (x_hi, x_lo), Ci, Ci, Fo, N_, kh, kw, taps, Ci, Fb=F_, b_f_add=crop,
-                bn=_conv_bn(Ci, -(-Co // 128) * kh * kw, out.device))
+                bn=_conv_bn(Ci, -(-Co // 128) * kh * kw, out.device), windows=windows)
     launch("dfold_taps_to_param", taps, Co, Ci, kh * kw, out, add)
 
 
-def conv5x5(x, weight, bias=None, relu: bool = True, residual=None, crop: int = 0):
+def _check_parts(op: str, name: str, value, total: int, what: str):
+    """``value`` (windows / segments) must be None or a positive integer that divides ``total`` (the leading axis)."""
+    if value is None:
+        return
+    if isinstance(value, bool) or not isinstance(value, int) or value < 1:
+        raise ValueError(f"{op}: {name} must be None or a positive integer, got {value!r}")
+    if total % value:
+        raise ValueError(f"{op}: {name}={value} does not divide the {total} {what}")
+
+
+def conv5x5(x, weight, bias=None, relu: bool = True, residual=None, crop: int = 0, windows: Optional[int] = None):
     """Channels-last ``Conv2d(kernel 5, padding 2)`` over the (frame, residue) image: x [F, N, C_in] ->
     ``relu?(conv(x) + bias) + residual`` [F, N, C_out]; weight keeps the reference's [C_out, C_in, 5, 5] layout.
-    ``crop > 0`` produces only the last ``F - crop`` output frames (residual must have that many frames)."""
-    return _Conv5x5Fn.apply(x, weight, bias, relu, residual, crop)
+    ``crop > 0`` produces only the last ``F - crop`` output frames (residual must have that many frames).
+
+    ``windows=W``: x stacks W windows of F / W frames each, [W * F_w, N, C_in], and each window is convolved on its own
+    (the frame halo stops at its edges, ``crop`` applies per window) in one launch per GEMM: the result equals W separate
+    calls bit for bit; the weight gradient is summed over the windows in one reduction."""
+    _check_parts("conv5x5", "windows", windows, x.shape[0], "frames")
+    if windows is not None and x.shape[0] // windows - crop < 1:
+        raise ValueError(f"conv5x5: crop={crop} removes every frame of the {x.shape[0] // windows}-frame windows")
+    return _Conv5x5Fn.apply(x, weight, bias, relu, residual, crop, windows)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -589,15 +626,19 @@ def conv5x5(x, weight, bias=None, relu: bool = True, residual=None, crop: int = 
 class _GlobalLNFn(Function):
     @staticmethod
     @_on_device
-    def forward(ctx, x, eps, silu):
+    def forward(ctx, x, eps, silu, segments):
         _need_cuda(x)
         xc = _f32c(x)
         y = torch.empty_like(xc)
-        stats = torch.empty(2, dtype=torch.float32, device=x.device)
-        ws = torch.empty(2048 + 2, dtype=torch.float64, device=x.device)
-        launch("dfold_global_layernorm_fwd", xc, y, stats, ws, xc.numel(), eps, int(silu))
+        S = segments or 1
+        stats = torch.empty(2 * S, dtype=torch.float32, device=x.device)
+        ws = torch.empty(S * (2048 + 2), dtype=torch.float64, device=x.device)
+        if segments is None:
+            launch("dfold_global_layernorm_fwd", xc, y, stats, ws, xc.numel(), eps, int(silu))
+        else:
+            launch("dfold_global_layernorm_seg_fwd", xc, y, stats, ws, xc.numel() // S, S, eps, int(silu))
         ctx.save_for_backward(xc, stats)
-        ctx.silu = silu
+        ctx.silu, ctx.segments = silu, segments
         return y
 
     @staticmethod
@@ -606,14 +647,24 @@ class _GlobalLNFn(Function):
         xc, stats = ctx.saved_tensors
         g = _f32c(dy)
         dx = torch.empty_like(xc)
-        ws = torch.empty(2048 + 2, dtype=torch.float64, device=xc.device)
-        launch("dfold_global_layernorm_bwd", xc, g, stats, ws, dx, xc.numel(), int(ctx.silu))
-        return dx, None, None
+        S = ctx.segments or 1
+        ws = torch.empty(S * (2048 + 2), dtype=torch.float64, device=xc.device)
+        if ctx.segments is None:
+            launch("dfold_global_layernorm_bwd", xc, g, stats, ws, dx, xc.numel(), int(ctx.silu))
+        else:
+            launch("dfold_global_layernorm_seg_bwd", xc, g, stats, ws, dx, xc.numel() // S, S, int(ctx.silu))
+        return dx, None, None, None
 
 
-def global_layernorm(x, eps: float = 1e-4, silu: bool = False):
-    """MyLayerNorm: one mean / unbiased variance over the whole tensor, optional fused SiLU."""
-    return _GlobalLNFn.apply(x, eps, silu)
+def global_layernorm(x, eps: float = 1e-4, silu: bool = False, segments: Optional[int] = None):
+    """MyLayerNorm: one mean / unbiased variance over the whole tensor, optional fused SiLU.
+
+    ``segments=S``: the leading axis holds S equal parts (one window each), each normalised with its own mean and
+    variance in one launch per pass; each part's result equals a call on that part alone bit for bit."""
+    _check_parts("global_layernorm", "segments", segments, x.shape[0] if x.dim() else 1, "rows of the leading axis")
+    if segments is not None and x.numel() // segments < 2:
+        raise ValueError(f"global_layernorm: each of the {segments} segments needs at least 2 elements")
+    return _GlobalLNFn.apply(x, eps, silu, segments)
 
 
 class _RowLNFn(Function):

@@ -25,6 +25,9 @@ comparable to the device time, so the step is:
   so an objective that needs its window's targets (``loss.score_network_loss``) reads slot i's in capture and in every
   replay; a loss function that returns ``(loss, aux_data)`` has slot 0's ``aux_data`` kept in static device tensors,
   ``aux``, overwritten by every step and never read back to the host;
+* ``batched=True`` trains the k windows of ``accumulate=k`` through one ``forward_windows`` pass of the network and one
+  backward of the sum of their losses, so the convolutions and the row-wise layers run on k times more rows per launch;
+  the optimizer step, ``loss`` and ``aux`` are those of ``accumulate=k`` (the gradient differs in fp32 summation order);
 * ``state_dict()`` / ``load_state_dict()`` save and resume the weights and the Adam(amsgrad) state in the reference
   trainer's checkpoint format, loading in place so the captured graph keeps running (checkpoint.py).
 """
@@ -91,7 +94,12 @@ class TrainStep:
     def __init__(self, net: torch.nn.Module, loss_fn: Callable[[Dict[str, torch.Tensor]], torch.Tensor],
                  example_feats: Dict[str, torch.Tensor], *, lr: float = 1e-4, world_size: int = 1, graph: bool = True,
                  warmup: int = 3, max_grad_norm: Optional[float] = None, lr_schedule: Optional[AlphaFoldSchedule] = None,
-                 accumulate: int = 1, loss_reads_window: bool = False):
+                 accumulate: int = 1, loss_reads_window: bool = False, batched: bool = False):
+        if not isinstance(batched, bool):
+            raise ValueError(f"batched must be True or False, got {batched!r}")
+        if batched and not callable(getattr(net, "forward_windows", None)):
+            raise ValueError(f"batched=True needs a network with forward_windows (FullScoreNetwork), got {type(net).__name__}")
+        self.batched = batched
         self.max_grad_norm = _check_max_grad_norm(max_grad_norm)
         if lr_schedule is not None and not isinstance(lr_schedule, AlphaFoldSchedule):
             raise ValueError(f"lr_schedule must be None or an AlphaFoldSchedule, got {type(lr_schedule).__name__}")
@@ -228,30 +236,58 @@ class TrainStep:
 
     def _eager(self):
         self.flat_grad.zero_()
-        for i, feats in enumerate(self.slots):
-            out = self.net(dict(feats))
-            loss = self.loss_fn(out, feats) if self.loss_reads_window else self.loss_fn(out)
-            if isinstance(loss, tuple):
-                loss, aux = loss
-                if i == 0:
-                    self._keep_aux(aux)
-                del aux
-            del out                                  # with the backward below, frees the window's activations before the next
-            prev, _kernels.GRAD_ACCUMULATE_INPLACE = _kernels.GRAD_ACCUMULATE_INPLACE, True     # wgrad kernels add into the flat buffer
-            try:
-                loss.backward()                      # AccumulateGrad adds into the param.grad views of the flat buffer
-            finally:
-                _kernels.GRAD_ACCUMULATE_INPLACE = prev
-                # the convolution weight gradients added on the side stream are complete before anything reads the buffer;
-                # joining once per window also frees the activation planes they read before the next window's forward
-                _kernels.join_side_stream()
-            if i == 0:
-                self.loss.copy_(loss.detach().float())
-            else:
-                self.loss.add_(loss.detach().float())
-            del loss
+        if self.batched:
+            self._windows_pass()
+        else:
+            self._window_loop()
         if self.accumulate > 1:
             self.loss.div_(self.accumulate)
+        self._reduce_and_update()
+
+    def _loss_of(self, i: int, out, feats) -> torch.Tensor:
+        """Window i's loss; its aux_data is kept when i == 0, and its value enters ``self.loss``."""
+        loss = self.loss_fn(out, feats) if self.loss_reads_window else self.loss_fn(out)
+        if isinstance(loss, tuple):
+            loss, aux = loss
+            if i == 0:
+                self._keep_aux(aux)
+            del aux
+        if i == 0:
+            self.loss.copy_(loss.detach().float())
+        else:
+            self.loss.add_(loss.detach().float())
+        return loss
+
+    def _backward(self, loss: torch.Tensor):
+        prev, _kernels.GRAD_ACCUMULATE_INPLACE = _kernels.GRAD_ACCUMULATE_INPLACE, True     # wgrad kernels add into the flat buffer
+        try:
+            loss.backward()                      # AccumulateGrad adds into the param.grad views of the flat buffer
+        finally:
+            _kernels.GRAD_ACCUMULATE_INPLACE = prev
+            # the convolution weight gradients added on the side stream are complete before anything reads the buffer
+            _kernels.join_side_stream()
+
+    def _windows_pass(self):
+        """batched=True: every slot's window through one forward_windows and one backward of the summed losses."""
+        outs = self.net.forward_windows([dict(feats) for feats in self.slots])
+        total = None
+        for i, (out, feats) in enumerate(zip(outs, self.slots)):
+            loss = self._loss_of(i, out, feats)
+            total = loss if total is None else total + loss
+            del loss
+        del outs, out
+        self._backward(total)
+
+    def _window_loop(self):
+        for i, feats in enumerate(self.slots):
+            out = self.net(dict(feats))
+            loss = self._loss_of(i, out, feats)
+            del out                                  # with the backward below, frees the window's activations before the next
+            # joining the side stream once per window also frees the activation planes it read before the next forward
+            self._backward(loss)
+            del loss
+
+    def _reduce_and_update(self):
         if self.world > 1 and self.opt is None and self.chunks > 1:
             # optional (DFOLD_ALLREDUCE_CHUNKS > 1): the gradient exchange in pieces, the Adam update of piece c running while
             # piece c + 1 is on the wire.  Smaller NCCL operations can lose more than the hidden Adam update gains, and

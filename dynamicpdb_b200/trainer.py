@@ -122,13 +122,20 @@ class Trainer:
     ``aux_losses=True`` trains on the objective with the backbone-atom and pair-distance losses added
     (``score_network_loss(aux_losses=True)``); ``experiment.bb_atom_loss_weight``, ``bb_atom_loss_t_filter``,
     ``dist_mat_loss_weight``, ``dist_mat_loss_t_filter`` and ``aux_loss_weight`` must then be numbers, and the log line
-    carries ``bb_atom_loss`` and ``dist_mat_loss`` too, in the reference's order."""
+    carries ``bb_atom_loss`` and ``dist_mat_loss`` too, in the reference's order.
+
+    ``batched=True`` trains each step's ``accumulate`` windows through one batched forward and backward
+    (``TrainStep(batched=True)``): the same windows in the same order, the same log line and checkpoints as
+    ``accumulate`` alone, with the gradient summed in another fp32 order."""
 
     def __init__(self, conf, net: torch.nn.Module, diffuser, *, world_size: int = 1, rank: int = 0, accumulate: int = 1,
                  graph: bool = True, warmup: int = 3, max_grad_norm: Optional[float] = None, lr_schedule=None,
-                 aux_losses: bool = False):
+                 aux_losses: bool = False, batched: bool = False):
+        if not isinstance(batched, bool):
+            raise ValueError(f"batched must be True or False, got {batched!r}")
         self._configure(conf, world_size, rank, accumulate, aux_losses=aux_losses)
-        self._build(net, diffuser, graph=graph, warmup=warmup, max_grad_norm=max_grad_norm, lr_schedule=lr_schedule)
+        self._build(net, diffuser, graph=graph, warmup=warmup, max_grad_norm=max_grad_norm, lr_schedule=lr_schedule,
+                    batched=batched)
         np.random.seed(rank)
         torch.manual_seed(rank)
 

@@ -98,6 +98,29 @@ int dfold_gemm_wgrad_bf16x3_bn(const uint16_t* a_hi, const uint16_t* a_lo, long 
                                long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
                                float* out, long ldo, float alpha, int bn, void* stream);
 
+/* dfold_gemm_bf16x3_bn over W >= 1 stacked windows of F frames each, each convolved on its own (the reference's
+ * nn.Conv2d stack, src/model/ipa_pytorch_dynamic.py:664-706, run once per window, as `world_size * W` one-window ranks
+ * of the released recipe train).  A planes [W][F][Nr][lda]; for w in [0, W), f in [0, F_out):
+ *   out[(w*F_out + f)*Nr + n, c] = act(alpha * sum_{tf,tn,k} A[w][f + f_start + tf - taps_f/2][n + tn - taps_n/2][k]
+ *                                      * B[tf*taps_n+tn][c][k] + bias[c]) + beta * residual[(w*F_out + f)*Nr + n, c]
+ * with A zero outside window w (the 4-D map's out-of-bounds fill).  Every output element is the same one-CTA k loop as
+ * dfold_gemm_bf16x3_bn on window w alone, so each window's result equals that call's bit for bit. */
+int dfold_gemm_bf16x3_windows(const uint16_t* a_hi, const uint16_t* a_lo, long W, long F, long F_out, int f_start, long Nr,
+                              long K, long lda, const uint16_t* b_hi, const uint16_t* b_lo, long n_out, long ldb,
+                              int taps_f, int taps_n, float* out, long ldo, const float* bias, const float* residual,
+                              long ldr, float alpha, float beta, int act, int bn, void* stream);
+
+/* Weight gradient over W >= 1 stacked windows (src/model/ipa_pytorch_dynamic.py:664-706, the gradient of the Conv2d
+ * weights summed over W windows):
+ *   out[t][m][n] = alpha * sum_w sum_{f,j} A[w][f][j][m] * B[w][f + b_f_add + tf - taps_f/2][j + tn - taps_n/2][n]
+ * A planes [W][F][Nr][lda], B planes [W][Fb][Nr][ldb], B zero outside window w.  One launch; the k loop runs window by
+ * window with the promotion points of one F*W-frame reduction, so it differs from the sum of W per-window gradients in
+ * fp32 rounding only.  bn = 64 or 128. */
+int dfold_gemm_wgrad_bf16x3_windows(const uint16_t* a_hi, const uint16_t* a_lo, long M, long lda,
+                                    const uint16_t* b_hi, const uint16_t* b_lo, long Nn, long ldb,
+                                    long W, long F, long Fb, int b_f_add, long Nr, int taps_f, int taps_n,
+                                    float* out, long ldo, float alpha, int bn, void* stream);
+
 /* Batched K-major GEMM (no taps).  For every row tile of "frame" b in [0, n_batches), hb = b % bmod:
  *   out[(b / o_f_div) * Nr + n, hb * o_col_bstride + c] =
  *       alpha * sum_k A[b / a_f_div][n][hb * a_k_bstride + k] * B[hb * b_z_bstride][c][b_k_ofs + hb * b_k_bstride + k]
@@ -142,6 +165,14 @@ int dfold_global_layernorm_fwd(const float* x, float* y, float* stats, double* w
                                void* stream);
 int dfold_global_layernorm_bwd(const float* x, const float* dy, const float* stats, double* workspace, float* dx,
                                long n, int silu, void* stream);
+/* MyLayerNorm (src/model/ipa_pytorch_dynamic.py:709-724) applied to each of `segments` consecutive tensors of n elements
+ * on its own (one window each), in one launch per pass: stats [segments][2]; workspace >= segments * 2050 doubles.
+ * Each segment is reduced with the partition and order dfold_global_layernorm_fwd / _bwd use for n elements, so its
+ * result equals that call's bit for bit. */
+int dfold_global_layernorm_seg_fwd(const float* x, float* y, float* stats, double* workspace, long n, int segments,
+                                   float eps, int silu, void* stream);
+int dfold_global_layernorm_seg_bwd(const float* x, const float* dy, const float* stats, double* workspace, float* dx,
+                                   long n, int segments, int silu, void* stream);
 /* nn.LayerNorm / openfold LayerNorm over the last axis (openfold/model/primitives.py:170-199). stats [rows][2].
  * dw, db must be pre-zeroed; they are accumulated in a fixed order, so they are the same from run to run. */
 int dfold_row_layernorm_fwd(const float* x, const float* w, const float* b, float* y, float* stats, long rows, int C,
