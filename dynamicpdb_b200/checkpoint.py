@@ -6,8 +6,11 @@ under DDP) and ``optimizer`` is ``torch.optim.Adam(model.parameters(), lr, amsgr
 ``state`` is keyed by the parameter's index in ``model.parameters()`` order and has no entry for a parameter that never
 received a gradient.  ``TrainStep`` keeps the same state in flat device buffers (the trained parameters back to back, padded
 to a multiple of four elements); the functions here map between those buffers, taken to the host, and that dict, and
-validate a dict before anything is written, so that a refused load leaves the step untouched.
+validate a dict before anything is written, so that a refused load leaves the step untouched.  A step that keeps a
+moving average of the weights (``TrainStep(ema_decay=...)``) adds OpenFold's ``ema`` entry,
+``ExponentialMovingAverage.state_dict()``.
 """
+import numbers
 import os
 import pickle
 import tempfile
@@ -89,16 +92,44 @@ def check_model(sd: dict, model_shapes: Dict[str, torch.Size]) -> Dict[str, torc
     the first tensor whose shape differs, so that a strict ``load_state_dict`` of the result cannot fail half-way."""
     if not isinstance(sd, dict) or not isinstance(sd.get("model"), dict):
         raise ValueError("checkpoint has no 'model' state_dict")
-    model = strip_module_prefix(sd["model"])
+    return _check_params(sd["model"], model_shapes, "model")
+
+
+def _check_params(params: dict, model_shapes: Dict[str, torch.Size], what: str) -> Dict[str, torch.Tensor]:
+    model = strip_module_prefix(params)
     unknown, missing = set(model) - set(model_shapes), set(model_shapes) - set(model)
     if unknown or missing:
-        raise ValueError(f"checkpoint model does not match the network: unknown keys [{_names(unknown)}], "
+        raise ValueError(f"checkpoint {what} does not match the network: unknown keys [{_names(unknown)}], "
                          f"missing keys [{_names(missing)}]")
     for k, shape in model_shapes.items():
         if not torch.is_tensor(model[k]) or tuple(model[k].shape) != tuple(shape):
             got = tuple(model[k].shape) if torch.is_tensor(model[k]) else type(model[k]).__name__
-            raise ValueError(f"checkpoint model '{k}' has shape {got}, the network {tuple(shape)}")
+            raise ValueError(f"checkpoint {what} '{k}' has shape {got}, the network {tuple(shape)}")
     return model
+
+
+def check_ema(sd: dict, model_shapes: Dict[str, torch.Size], decay: Optional[float] = None
+              ) -> Optional[Dict[str, torch.Tensor]]:
+    """Validates the ``ema`` entry of a checkpoint dict, OpenFold's ``ExponentialMovingAverage.state_dict()``
+    (``{'params': the averaged net.state_dict(), 'decay': float}``), and returns its tensors by the network's own names
+    (``module.`` stripped), or None when the checkpoint has no ``ema``.  Raises ValueError for unknown or missing keys, a
+    shape that differs, a tensor that is not float32, or, when ``decay`` is given, a decay other than it."""
+    ema = sd.get("ema") if isinstance(sd, dict) else None
+    if ema is None:
+        return None
+    if not isinstance(ema, dict) or not isinstance(ema.get("params"), dict):
+        raise ValueError("checkpoint ema has no 'params' state_dict")
+    d = ema.get("decay")
+    if isinstance(d, bool) or not isinstance(d, numbers.Real):
+        raise ValueError(f"checkpoint ema decay must be a number, got {d!r}")
+    params = _check_params(ema["params"], model_shapes, "ema")
+    for k in model_shapes:
+        if params[k].dtype != torch.float32:
+            raise ValueError(f"checkpoint ema '{k}' is {params[k].dtype}; the average is kept in torch.float32")
+    if decay is not None and float(d) != decay:
+        raise ValueError(f"checkpoint ema decay {d!r} differs from the training step's {decay!r}: construct "
+                         f"TrainStep(ema_decay={d!r}) to resume this checkpoint")
+    return params
 
 
 def check_state(sd: dict, layout: FlatLayout, model_shapes: Dict[str, torch.Size], lr: float, schedule=None
@@ -180,10 +211,13 @@ def optimizer_to_flat(layout: FlatLayout, entries: Optional[Dict[int, dict]]) ->
 
 def save_checkpoint(path: str, train_step, conf, epoch: int, step: int) -> None:
     """Writes ``du.write_checkpoint``'s dict ``{'model', 'conf', 'optimizer', 'epoch', 'step'}`` for ``train_step``
-    (``conf`` as given: the evaluator reads ``conf.model``).  The file is written next to ``path`` under a temporary name
+    (``conf`` as given: the evaluator reads ``conf.model``), and ``ema`` after them when the step keeps a moving average
+    of the weights, as OpenFold's checkpoints carry it.  The file is written next to ``path`` under a temporary name
     and renamed onto it, so an interrupted save leaves the previous checkpoint in place."""
     sd = train_step.state_dict()
     ckpt = {"model": sd["model"], "conf": conf, "optimizer": sd["optimizer"], "epoch": epoch, "step": step}
+    if "ema" in sd:
+        ckpt["ema"] = sd["ema"]
     d = os.path.dirname(os.path.abspath(path))
     fd, tmp = tempfile.mkstemp(dir=d, prefix=os.path.basename(path) + ".", suffix=".tmp")
     try:

@@ -715,6 +715,21 @@ __global__ void __launch_bounds__(256) adam_amsgrad_kernel(float* __restrict__ p
     }
 }
 
+// OpenFold's ExponentialMovingAverage._update_state_dict_ (openfold/utils/exponential_moving_average.py:40-49):
+// diff = stored - param; diff *= 1 - decay; stored -= diff.  Three fp32 roundings with explicit intrinsics, so the update
+// is never contracted into an FMA and gives torch's bits; c is fp32(1 - decay), the factor torch's mul_ applies.
+__global__ void __launch_bounds__(256) ema_update_kernel(float* __restrict__ ema, const float* __restrict__ p, long n4, float c) {
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
+        float4 E = reinterpret_cast<float4*>(ema)[i];
+        const float4 P = reinterpret_cast<const float4*>(p)[i];
+        E.x = __fsub_rn(E.x, __fmul_rn(__fsub_rn(E.x, P.x), c));
+        E.y = __fsub_rn(E.y, __fmul_rn(__fsub_rn(E.y, P.y), c));
+        E.z = __fsub_rn(E.z, __fmul_rn(__fsub_rn(E.z, P.z), c));
+        E.w = __fsub_rn(E.w, __fmul_rn(__fsub_rn(E.w, P.w), c));
+        reinterpret_cast<float4*>(ema)[i] = E;
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------
 // Global L2 norm of the flat gradient and the clipping coefficient of torch.nn.utils.clip_grad_norm_ (norm_type 2), the
 // optimizer-side option of the reference trainer (train_DFOLD_dynamics.py:665).  The order of the sum depends on n only, not
@@ -790,16 +805,21 @@ __global__ void lr_schedule_kernel(const float* __restrict__ step, double base_l
 }
 }  // namespace
 
+// The grid of the float4 grid-stride passes over flat buffers: 16 CTAs of 256 threads per SM, grid-stride beyond.
+static int flat_pass_blocks(long n4) {
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
+        sms = 132;
+    const long cap = 16L * sms;
+    return (int)(cdiv(n4, 256) < cap ? cdiv(n4, 256) : cap);
+}
+
 static int adam_launch(bool clip, float* param, const float* grad, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq,
                        long n, float* step, int tick, float lr, float beta1, float beta2, float eps, float grad_scale,
                        const float* coef, const float* dlr, cudaStream_t st) {
     if (tick) adam_tick_kernel<<<1, 1, 0, st>>>(step);            // chunked callers advance the step once per optimizer step
     const long n4 = n / 4;
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-        sms = 132;
-    const long cap = 16L * sms;                                     // 16 CTAs of 256 threads per SM, grid-stride beyond
-    const int blocks = (int)(cdiv(n4, 256) < cap ? cdiv(n4, 256) : cap);
+    const int blocks = flat_pass_blocks(n4);
 #define DFOLD_ADAM(CLIP, DLR)                                                                                                  \
     adam_amsgrad_kernel<CLIP, DLR><<<blocks, 256, 0, st>>>(param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n4, step, lr, beta1, \
                                                            beta2, eps, grad_scale, coef, dlr)
@@ -838,6 +858,16 @@ extern "C" int dfold_adam_amsgrad_dlr(float* param, const float* grad, float* ex
     DFOLD_REQUIRE(lr != nullptr, "dfold_adam_amsgrad_dlr: null learning rate");
     return dfold::adam_launch(coef != nullptr, param, grad, exp_avg, exp_avg_sq, max_exp_avg_sq, n, step, tick, 0.f, beta1, beta2,
                               eps, grad_scale, coef, lr, dfold::as_stream(stream));
+}
+
+// n must be a multiple of 4 and the buffers 16-byte aligned, as for Adam.
+extern "C" int dfold_ema_update(float* ema, const float* param, long n, float one_minus_decay, void* stream) {
+    DFOLD_REQUIRE(n > 0 && n % 4 == 0, "dfold_ema_update: n must be a positive multiple of 4");
+    DFOLD_REQUIRE(ema != nullptr && param != nullptr, "dfold_ema_update: null buffer");
+    DFOLD_REQUIRE(one_minus_decay >= 0.f && one_minus_decay <= 1.f, "dfold_ema_update: 1 - decay must lie in [0, 1]");
+    const long n4 = n / 4;
+    dfold::ema_update_kernel<<<dfold::flat_pass_blocks(n4), 256, 0, dfold::as_stream(stream)>>>(ema, param, n4, one_minus_decay);
+    return dfold::check_launch("ema_update_kernel");
 }
 
 extern "C" int dfold_lr_schedule(const float* step, double base_lr, double max_lr, long warmup_no_steps,

@@ -59,14 +59,22 @@ def eval_seeds(seed: int) -> Tuple[int, int]:
     return tuple(int(s.generate_state(1, np.uint64)[0]) for s in np.random.SeedSequence(seed).spawn(2))
 
 
-def load_weights(net: torch.nn.Module, path: str) -> None:
+def load_weights(net: torch.nn.Module, path: str, ema: bool = False) -> None:
     """Loads ``path``'s ``model`` state_dict into ``net`` strictly, ``module.`` prefixes stripped, as the reference
     evaluator's ``_load_ckpt`` does (eval_DFOLD_dynamics.py:131-136): a checkpoint of ``checkpoint.save_checkpoint`` or of
-    the reference trainer.  Every key and shape is checked first (``checkpoint.check_model``), so a mismatch raises
-    ValueError and leaves ``net`` as it was.  Checkpoints are trusted input: ``conf`` is an arbitrary pickled object, so the
-    file is read with ``weights_only=False`` as the reference does; never load one from an untrusted source."""
+    the reference trainer.  ``ema=True`` loads the moving average of the weights instead, ``ema['params']`` of a checkpoint
+    written with ``TrainStep(ema_decay=...)`` (OpenFold's layout), and raises ValueError naming the file when it has none.
+    Every key and shape is checked first (``checkpoint.check_model`` / ``check_ema``), so a mismatch raises ValueError and
+    leaves ``net`` as it was.  Checkpoints are trusted input: ``conf`` is an arbitrary pickled object, so the file is read
+    with ``weights_only=False`` as the reference does; never load one from an untrusted source."""
     ckpt = torch.load(path, map_location="cpu", weights_only=False)
-    model = _ckpt.check_model(ckpt, {k: v.shape for k, v in net.state_dict().items()})
+    shapes = {k: v.shape for k, v in net.state_dict().items()}
+    if ema:
+        model = _ckpt.check_ema(ckpt, shapes)
+        if model is None:
+            raise ValueError(f"{path}: the checkpoint has no 'ema' (moving average of the weights) to evaluate")
+    else:
+        model = _ckpt.check_model(ckpt, shapes)
     net.load_state_dict(model, strict=True)
 
 
@@ -90,16 +98,19 @@ class Evaluator:
     define); ``experiment.noise_scale``.  Everything is checked, and the csv read, before the checkpoint is read and before
     any device work.  ``net`` is built by the caller (from the checkpoint's ``conf.model`` where it has one) with a
     ``score_epilogue.SE3ScoreDiffuser``; ``diffuser`` is the one the windows' ``sample_ref`` draws from.  The weights are
-    loaded into ``net`` in the constructor and ``net`` is put in eval mode.
+    loaded into ``net`` in the constructor and ``net`` is put in eval mode; ``ema=True`` loads the checkpoint's moving
+    average of the weights (``load_weights``), so ``evaluate`` and ``extend`` run on it.
 
     Random streams: two CUDA generators seeded from ``seed`` (``eval_seeds``), one for the windows' ``sample_ref`` (drawn by
     the prefetcher's worker thread), one for the reverse steps (drawn by the calling thread), so a run is reproducible bit
     for bit whatever the threads' timing.  The global generators are not touched.  The reference draws both from numpy's
     global stream on the host; those numbers are not reproduced."""
 
-    def __init__(self, conf, net: torch.nn.Module, diffuser, *, seed: int = 0, depth: int = 2):
+    def __init__(self, conf, net: torch.nn.Module, diffuser, *, seed: int = 0, depth: int = 2, ema: bool = False):
+        if not isinstance(ema, bool):
+            raise ValueError(f"ema must be True or False, got {ema!r}")
         self._configure(conf)
-        load_weights(net, self.weights_path)
+        load_weights(net, self.weights_path, ema=ema)
         net.eval()
         self.net, self.diffuser, self.seed, self.depth = net, diffuser, int(seed), depth
         self.device = next(net.parameters()).device

@@ -69,6 +69,7 @@ _SIGS = {
     "dfold_grad_norm": "plff" + "ppp" + "p",
     "dfold_adam_amsgrad_dlr": "pppppl" + "pi" + "p" + "ffff" + "pp",
     "dfold_lr_schedule": "p" + "dd" + "lll" + "d" + "pp",
+    "dfold_ema_update": "pplf" + "p",
     "dfold_featurize_window": "pppppp" + "ii" + "pppp" + "p",
     "dfold_loss_fwd": "pppppppppppp" + "ii" + "dddd" + "ii" + "pppp" + "p",
     "dfold_aux_loss_fwd": "ppppp" + "iii" + "ddddd" + "pppp" + "p",

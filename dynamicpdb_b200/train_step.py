@@ -29,8 +29,12 @@ comparable to the device time, so the step is:
   backward of the sum of their losses, so the convolutions and the row-wise layers run on k times more rows per launch;
   the optimizer step, ``loss`` and ``aux`` are those of ``accumulate=k`` (the gradient differs in fp32 summation order);
 * ``state_dict()`` / ``load_state_dict()`` save and resume the weights and the Adam(amsgrad) state in the reference
-  trainer's checkpoint format, loading in place so the captured graph keeps running (checkpoint.py).
+  trainer's checkpoint format, loading in place so the captured graph keeps running (checkpoint.py);
+* ``ema_decay=d`` keeps OpenFold's exponential moving average of the weights (``ExponentialMovingAverage``,
+  openfold/utils/exponential_moving_average.py, d = 0.999 in its config) in a flat buffer, ``ema``, updated by one
+  ``dfold_ema_update`` launch inside the graph after every optimizer step and saved as the checkpoint's ``ema`` entry.
 """
+import collections
 import dataclasses
 import math
 import copy
@@ -94,7 +98,8 @@ class TrainStep:
     def __init__(self, net: torch.nn.Module, loss_fn: Callable[[Dict[str, torch.Tensor]], torch.Tensor],
                  example_feats: Dict[str, torch.Tensor], *, lr: float = 1e-4, world_size: int = 1, graph: bool = True,
                  warmup: int = 3, max_grad_norm: Optional[float] = None, lr_schedule: Optional[AlphaFoldSchedule] = None,
-                 accumulate: int = 1, loss_reads_window: bool = False, batched: bool = False):
+                 accumulate: int = 1, loss_reads_window: bool = False, batched: bool = False,
+                 ema_decay: Optional[float] = None):
         if not isinstance(batched, bool):
             raise ValueError(f"batched must be True or False, got {batched!r}")
         if batched and not callable(getattr(net, "forward_windows", None)):
@@ -109,6 +114,10 @@ class TrainStep:
         self.accumulate = int(accumulate)
         self.fused_adam = os.environ.get("DFOLD_TORCH_ADAM", "0") != "1"
         self.chunks = max(1, int(os.environ.get("DFOLD_ALLREDUCE_CHUNKS", "1")))
+        self.ema_decay = check_ema_decay(ema_decay)
+        if self.ema_decay is not None and not self.fused_adam:
+            raise ValueError("ema_decay averages the fused optimizer's flat parameter buffer, which DFOLD_TORCH_ADAM=1 "
+                             "does not have: unset it to keep a moving average")
         if self.max_grad_norm is not None and self.fused_adam and world_size > 1 and self.chunks > 1:
             raise ValueError("max_grad_norm needs the whole all-reduced gradient before the first update, but "
                              f"DFOLD_ALLREDUCE_CHUNKS={self.chunks} updates each piece as soon as it is reduced: "
@@ -154,6 +163,12 @@ class TrainStep:
             if self.current_lr is not None:
                 self.current_lr = self.opt.param_groups[0]["lr"]           # the tensor the optimizer reads
                 self._step0 = torch.zeros((), dtype=torch.float32, device=dev)    # the step count before Adam has state
+        # OpenFold's moving average of the weights over the flat layout (padding stays 0), starting from the weights
+        # handed in.  Torch's ``diff *= 1 - decay`` multiplies the fp32 tensor by fp32(1 - decay), 1 - decay in double.
+        self.ema: Optional[torch.Tensor] = None
+        if self.ema_decay is not None:
+            self.ema = self.flat_param.clone()
+            self.ema_factor = 1.0 - self.ema_decay
         # one set of static input buffers per accumulated window
         self.slots = [{k: v.clone() for k, v in example_feats.items()} for _ in range(self.accumulate)]
         self.static = self.slots[0]
@@ -208,6 +223,8 @@ class TrainStep:
         with torch.no_grad():
             for p, v in zip(self.params, saved_params):
                 p.copy_(v)
+            if self.ema is not None:
+                self.ema.copy_(self.flat_param)
             if self.opt is None:
                 for t in (self.exp_avg, self.exp_avg_sq, self.max_exp_avg_sq, self.step_count):
                     t.zero_()
@@ -306,6 +323,9 @@ class TrainStep:
             if self.opt is not None and self.grad_scale != 1.0:
                 self.flat_grad.mul_(self.grad_scale)        # (the fused optimizer scales the summed gradient on the fly)
             self.optimizer_step()
+        if self.ema is not None:
+            # after the whole update, every piece of it; each rank averages the same weights, so no collective
+            _kernels.launch("dfold_ema_update", self.ema, self.flat_param, self.ema.numel(), self.ema_factor)
 
     def _keep_aux(self, aux: Dict[str, torch.Tensor]):
         if self.aux is None:
@@ -379,8 +399,9 @@ class TrainStep:
 
     def state_dict(self) -> Dict[str, object]:
         """``{'model': net.state_dict() on the host, 'optimizer': torch.optim.Adam(net.parameters(), lr,
-        amsgrad=True).state_dict()}`` (checkpoint.py).  Each flat buffer is copied to the host once; the per-parameter
-        tensors are views of those copies."""
+        amsgrad=True).state_dict()}`` (checkpoint.py), and with ``ema_decay`` ``'ema':
+        ExponentialMovingAverage.state_dict()``, ``{'params': the averaged net.state_dict(), 'decay': ema_decay}``.  Each
+        flat buffer is copied to the host once; the per-parameter tensors are views of those copies."""
         if self.opt is None:
             flat = [t.cpu() for t in (self.flat_param, self.exp_avg, self.exp_avg_sq, self.max_exp_avg_sq)]
             step = float(self.step_count)
@@ -394,17 +415,28 @@ class TrainStep:
             opt = _ckpt.optimizer_state_dict(self.layout, *flat[1:], step, self.lr)
         else:       # the lr the next step uses, and the optimizer's lr from before the scheduler, as LRScheduler leaves them
             opt = _ckpt.optimizer_state_dict(self.layout, *flat[1:], step, self.schedule.lr(int(step)), initial_lr=self.lr)
-        return {"model": model, "optimizer": opt}
+        sd = {"model": model, "optimizer": opt}
+        if self.ema is not None:
+            # ExponentialMovingAverage.state_dict(): the average of every net.state_dict() entry; the average of an entry
+            # the step does not train is that entry's constant value
+            avg = {n: v for n, v in zip(self.layout.names, _ckpt.views(self.layout, self.ema.cpu())) if v is not None}
+            params = collections.OrderedDict((k, avg[k] if k in avg else v.detach().cpu().clone())
+                                             for k, v in self.net.state_dict().items())
+            sd["ema"] = collections.OrderedDict(params=params, decay=self.ema_decay)
+        return sd
 
     def load_state_dict(self, sd: Dict[str, object]) -> None:
         """Loads ``state_dict()``'s dict or a checkpoint of the reference trainer (``module.`` prefixes, a non-capturable
         optimizer's CPU ``step``) IN PLACE: the captured graph holds pointers to the parameter, moment and step buffers,
         and keeps replaying them.  No ``optimizer`` (or None) is a weights-only warm start with zero moments and step.
+        With ``ema_decay`` the checkpoint's ``ema`` is loaded too (checkpoint.check_ema: its decay must be the step's), and
+        a checkpoint without one starts the average from its weights; a step without ``ema_decay`` ignores ``ema``.
         Everything is validated before the first write (checkpoint.check_state): a refused load raises ValueError and
         leaves the step as it was.  Every data-parallel rank loads the same file, so no collective is needed.  With a
         schedule, the checkpoint's lr must be the schedule's lr at its step: a run saved under another schedule is refused."""
-        model, entries, step = _ckpt.check_state(sd, self.layout, {k: v.shape for k, v in self.net.state_dict().items()},
-                                                 self.lr, self.schedule)
+        shapes = {k: v.shape for k, v in self.net.state_dict().items()}
+        model, entries, step = _ckpt.check_state(sd, self.layout, shapes, self.lr, self.schedule)
+        ema = None if self.ema is None else _ckpt.check_ema(sd, shapes, self.ema_decay)
         moments = _ckpt.optimizer_to_flat(self.layout, entries)
         trained = {n for n, o in zip(self.layout.names, self.layout.offsets) if o is not None}
         with torch.no_grad():
@@ -413,6 +445,10 @@ class TrainStep:
                 for buf, m in zip((self.exp_avg, self.exp_avg_sq, self.max_exp_avg_sq), moments):
                     buf.copy_(m)
                 self.step_count.fill_(step)
+                if self.ema is not None:
+                    # without an average in the checkpoint it starts from the loaded weights, as a fresh
+                    # ExponentialMovingAverage(model) would
+                    self.ema.copy_(self.flat_param if ema is None else _ckpt.model_to_flat(self.layout, ema))
             else:
                 per = [[v for v in _ckpt.views(self.layout, m) if v is not None] for m in moments]
                 for j, p in enumerate(self.params):
@@ -427,6 +463,15 @@ class TrainStep:
                 self.current_lr.fill_(self.schedule.lr(int(step)))
         _kernels.invalidate_weight_cache()          # no bf16 weight plane from before the load may be reused
         torch.cuda.synchronize()
+
+
+def check_ema_decay(v) -> Optional[float]:
+    """None (no moving average), or the decay of OpenFold's ExponentialMovingAverage, a number in [0, 1]."""
+    if v is None:
+        return None
+    if isinstance(v, bool) or not isinstance(v, numbers.Real) or not 0.0 <= float(v) <= 1.0:      # (NaN fails too)
+        raise ValueError(f"ema_decay must be None or a number in [0, 1], got {v!r}")
+    return float(v)
 
 
 def _check_max_grad_norm(v) -> Optional[float]:

@@ -27,7 +27,7 @@ from torch.utils.data.distributed import DistributedSampler
 from . import checkpoint as _ckpt
 from .input_pipeline import TrajectoryStore, WindowPrefetcher
 from .loss import AUX_KEYS, aux_conf, score_network_loss
-from .train_step import TrainStep
+from .train_step import TrainStep, check_ema_decay
 
 ROW_FIELDS = ("atlas_npz", "force_path", "vel_path", "embed_path")
 LOGGED = ("total_loss", "rot_loss", "trans_loss", "torsion_loss")     # score_network_loss's aux_data keys without 'batch'
@@ -126,16 +126,20 @@ class Trainer:
 
     ``batched=True`` trains each step's ``accumulate`` windows through one batched forward and backward
     (``TrainStep(batched=True)``): the same windows in the same order, the same log line and checkpoints as
-    ``accumulate`` alone, with the gradient summed in another fp32 order."""
+    ``accumulate`` alone, with the gradient summed in another fp32 order.
+
+    ``ema_decay=d`` keeps OpenFold's moving average of the weights (``TrainStep(ema_decay=d)``); the checkpoints then
+    carry it as ``ema`` and ``resume`` restores it."""
 
     def __init__(self, conf, net: torch.nn.Module, diffuser, *, world_size: int = 1, rank: int = 0, accumulate: int = 1,
                  graph: bool = True, warmup: int = 3, max_grad_norm: Optional[float] = None, lr_schedule=None,
-                 aux_losses: bool = False, batched: bool = False):
+                 aux_losses: bool = False, batched: bool = False, ema_decay: Optional[float] = None):
         if not isinstance(batched, bool):
             raise ValueError(f"batched must be True or False, got {batched!r}")
+        check_ema_decay(ema_decay)
         self._configure(conf, world_size, rank, accumulate, aux_losses=aux_losses)
         self._build(net, diffuser, graph=graph, warmup=warmup, max_grad_norm=max_grad_norm, lr_schedule=lr_schedule,
-                    batched=batched)
+                    batched=batched, ema_decay=ema_decay)
         np.random.seed(rank)
         torch.manual_seed(rank)
 

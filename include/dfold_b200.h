@@ -408,6 +408,13 @@ int dfold_adam_amsgrad_dlr(float* param, const float* grad, float* exp_avg, floa
  * start_decay_after_n_steps, decay_every_n_steps > 0 and a finite max_lr > 0. */
 int dfold_lr_schedule(const float* step, double base_lr, double max_lr, long warmup_no_steps, long start_decay_after_n_steps,
                       long decay_every_n_steps, double decay_factor, float* lr, void* stream);
+/* One update of OpenFold's exponential moving average of the weights (ExponentialMovingAverage._update_state_dict_,
+ * openfold/utils/exponential_moving_average.py:40-49, decay 0.999 in openfold/config.py:493) over flat fp32 buffers of n
+ * elements (n % 4 == 0, 16-byte aligned):
+ *   diff = ema - param;  diff *= one_minus_decay;  ema -= diff
+ * each operation rounded to fp32 on its own (never an FMA), which gives the bits of those three torch ops when
+ * one_minus_decay = fp32(1 - decay), 1 - decay taken in double as Python does.  0 <= one_minus_decay <= 1. */
+int dfold_ema_update(float* ema, const float* param, long n, float one_minus_decay, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Evaluation metrics (csrc/metrics.cu), SURVEY.md 8 f6: the arithmetic of Experiment.eval_fn (train_DFOLD_dynamics.py:
